@@ -577,6 +577,10 @@ int b200sph_column_counts(b200sph_ctx *ctx, int arr, double x0, double inv_width
 /* ---- bookkeeping -------------------------------------------------------- */
 int b200sph_get_stats(b200sph_ctx *ctx, b200sph_stats *out);
 int b200sph_reset_stats(b200sph_ctx *ctx);
+/* how many of the stats' pair_launches (since the last reset) read the 32-byte records
+ * (k_pair_list_r32: the WCSPH Group, uniform h and m, one Tait EOS with gamma = 7, no
+ * ghosts; B200SPH_RECORDS=48 turns them off) */
+int b200sph_records32_launches(b200sph_ctx *ctx, int64_t *out);
 /* per-phase CUDA-event timing: 0 off, 1 every phase (ms_nnps, ms_pair, ms_other),
  * 2 the pair kernels only (ms_pair; two events per pair pass instead of ~25 per
  * step).  Event pairs are recorded on the stream (no sync) and resolved by

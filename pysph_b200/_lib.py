@@ -216,6 +216,7 @@ SIGNATURES = {
                                         C.c_void_p]),
     'b200sph_get_stats': (C.c_int, [_ctx_p, C.POINTER(Stats)]),
     'b200sph_reset_stats': (C.c_int, [_ctx_p]),
+    'b200sph_records32_launches': (C.c_int, [_ctx_p, C.POINTER(_i64)]),
     'b200sph_set_profiling': (C.c_int, [_ctx_p, C.c_int]),
 }
 

@@ -139,6 +139,19 @@ __host__ __device__ static inline void tait_powers(const double ratio, const dou
     }
 }
 
+// The 32-byte record of the WCSPH pass when h, m and the Tait EOS (gamma = 7) are the same for
+// every particle (records32 in b200sph.cu): R = {(x, y, z, delta), (u, v, w, type)} with
+// delta = rho / rho0 - 1 formed in fp64 after the clamp of TaitEOSHGCorrection, so that fp32
+// keeps the digits of the density variation; k_pair_list_r32 recomputes rho, p / rho^2 and cs
+// from delta.  ONE function for every writer, so that they all produce the same bits.
+__device__ __forceinline__ void rec32_make(const float4 A, const double u, const double v, const double w, double rho,
+                                           const bool clamp, const double rho0, const int type, float4 &R0, float4 &R1)
+{
+    if (clamp && rho < rho0) rho = rho0;
+    R0 = make_float4(A.x, A.y, A.z, (float)(rho * (1.0 / rho0) - 1.0));
+    R1 = make_float4((float)u, (float)v, (float)w, __int_as_float(type));
+}
+
 struct PendingEvent {
     cudaEvent_t e0, e1;
     int slot;  // 0 nnps, 1 pair, 2 other
@@ -207,6 +220,18 @@ struct b200sph_ctx {
     uint32_t *perm_tmp = nullptr, *perm = nullptr, *skey = nullptr, *rank = nullptr;
     float4 *A = nullptr, *B = nullptr, *C = nullptr;
     float4 *AB = nullptr;  // {A, B} interleaved (32 B = one sector per particle) for the list consumer's 256-bit gathers
+    // the 32-byte records of the WCSPH pass (records32): {(x, y, z, rho / rho0 - 1), (u, v, w, type)};
+    // while rec32 holds, the state records are packed HERE instead of B / C / the B half of AB
+    float4 *R = nullptr;
+    bool rec32 = false;
+    double rec32_rho0 = 0.0;    // the rho0 of the packed delta
+    bool ab_stale = false;      // k_stage_pack wrote the positions into R only (ab_positions restores AB)
+    bool rec48_forced = false;  // env B200SPH_RECORDS=48
+    // h and m over all particles (records32 needs both uniform): computed on demand by one
+    // min/max reduction, cleared by set_changed / h_changed / m_changed
+    bool hm_known = false;
+    double h_uniform = NAN, m_uniform = NAN;   // NaN: not uniform
+    int64_t n_pair_r32 = 0;
     int64_t n_sorted = 0;
     bool state_packed = false;
     int force_kernel = 0;       // 0 lists (default), 1 warp kernel (env B200SPH_PAIR_KERNEL)
@@ -339,8 +364,16 @@ struct b200sph_ctx {
 // ghost repacks).
 
 // Positions or h of the same particles changed: the grid and the packed positions are stale.
-// The build may survive: nnps_update measures the drift against it.
-static void positions_changed(b200sph_ctx *ctx) { ctx->grid_valid = false, ctx->packed_valid = false; }
+// The build may survive: nnps_update measures the drift against it.  The 32-byte records
+// carry the positions as well: only k_stage_pack rewrites them with the positions (and says
+// so); the next nnps_update rewrites the position half of AB, unless k_stage_pack did (then
+// it sets ab_stale again).
+static void positions_changed(b200sph_ctx *ctx)
+{
+    ctx->grid_valid = false, ctx->packed_valid = false;
+    if (ctx->rec32) ctx->state_packed = false;
+    ctx->ab_stale = false;
+}
 
 // A property the pair records (B, C) are made of changed, or B / C now hold other records:
 // the next pair pass packs them again.
@@ -358,7 +391,12 @@ static void h_changed(b200sph_ctx *ctx)
 {
     positions_changed(ctx);
     ctx->domain_valid = false, ctx->h_dirty = true;
+    ctx->hm_known = false;
 }
+
+// m changed (a push, or a generic Group that stores to the state): records32 must look at
+// the masses again.
+static void m_changed(b200sph_ctx *ctx) { ctx->hm_known = false; }
 
 // The build cannot be reused (domain, mirror planes or kernel support changed, or a deferred
 // drift check failed): the next nnps_update makes a full build, which repacks the state.
@@ -379,6 +417,7 @@ static void set_changed(b200sph_ctx *ctx)
     build_invalid(ctx);
     state_changed(ctx);
     ctx->ptype_dirty = true, ctx->h_dirty = true;
+    ctx->hm_known = false;
 }
 
 // Particles arrived or left with their own h (halo_append, migrate_out, mirror images): the
@@ -647,6 +686,7 @@ static int pool_layout(b200sph_ctx *ctx, const int64_t *new_cap)
     if (ctx->B) cudaFree(ctx->B);
     if (ctx->C) cudaFree(ctx->C);
     if (ctx->AB) cudaFree(ctx->AB);
+    if (ctx->R) cudaFree(ctx->R);
     if (ctx->A0) cudaFree(ctx->A0);
     if (ctx->Dv) cudaFree(ctx->Dv);
     if (ctx->PT) cudaFree(ctx->PT);
@@ -663,6 +703,7 @@ static int pool_layout(b200sph_ctx *ctx, const int64_t *new_cap)
     CU(cudaMalloc((void **)&ctx->B, 16 * (size_t)alloc));
     CU(cudaMalloc((void **)&ctx->C, 16 * (size_t)alloc));
     CU(cudaMalloc((void **)&ctx->AB, 32 * (size_t)alloc));
+    CU(cudaMalloc((void **)&ctx->R, 32 * (size_t)alloc));
     CU(cudaMalloc((void **)&ctx->A0, 16 * (size_t)alloc));
     CU(cudaMalloc((void **)&ctx->Dv, 16 * (size_t)alloc));
     CU(cudaMalloc((void **)&ctx->PT, 8 * (size_t)alloc));
@@ -904,6 +945,7 @@ int b200sph_create(int device, b200sph_ctx **out)
     if (const char *e = getenv("B200SPH_PROACTIVE")) ctx->proactive = atoi(e) != 0;
     if (const char *e = getenv("B200SPH_SKIN")) ctx->skin = ctx->skin_max = std::max(0.0, atof(e));
     if (const char *e = getenv("B200SPH_SKIN_ADAPT")) ctx->skin_adapt = atoi(e) != 0;
+    if (const char *e = getenv("B200SPH_RECORDS")) ctx->rec48_forced = atoi(e) == 48;
     ctx->skin_min = std::min(ctx->skin_min, ctx->skin_max);
     CU(cudaMalloc((void **)&ctx->red_u32, 4 * sizeof(unsigned)));
     CU(cudaMallocHost((void **)&ctx->red_u32_host, 4 * sizeof(unsigned)));
@@ -936,7 +978,7 @@ int b200sph_destroy(b200sph_ctx *ctx)
     cudaFree(ctx->ptype);
     cudaFree(ctx->key_of); cudaFree(ctx->off_in); cudaFree(ctx->cell_cnt); cudaFree(ctx->cell_start);
     cudaFree(ctx->blk_sums); cudaFree(ctx->perm_tmp); cudaFree(ctx->perm); cudaFree(ctx->skey);
-    cudaFree(ctx->rank); cudaFree(ctx->A); cudaFree(ctx->B); cudaFree(ctx->C); cudaFree(ctx->AB);
+    cudaFree(ctx->rank); cudaFree(ctx->A); cudaFree(ctx->B); cudaFree(ctx->C); cudaFree(ctx->AB); cudaFree(ctx->R);
     cudaFree(ctx->red); cudaFreeHost(ctx->red_host); cudaFree(ctx->counter);
     cudaFreeHost(ctx->counter_host); cudaFree(ctx->stage_buf); cudaFree(ctx->flag_a);
     cudaFree(ctx->flag_b); cudaFree(ctx->A0); cudaFree(ctx->lst); cudaFree(ctx->cnt);
@@ -1129,6 +1171,7 @@ int b200sph_push_f64(b200sph_ctx *ctx, int arr, int prop, const double *host, in
     // measures the drift against the current neighbour build and reuses it if it can
     if (prop == B200SPH_H) h_changed(ctx);
     else if (prop <= B200SPH_Z) positions_changed(ctx);
+    else if (prop == B200SPH_M) m_changed(ctx);
     state_changed(ctx);
     return 0;
 }
@@ -1325,6 +1368,29 @@ static int run_minmax(b200sph_ctx *ctx, int do_xyz, int do_h)
     return 0;
 }
 
+// h and m of every particle uniform?  k_reduce_minmax over (h, m, m) into slots 0..5 only:
+// the dt factors a fused stage2 may have reduced into slots 9, 11, 12 stay where they are
+static int hm_uniformity(b200sph_ctx *ctx)
+{
+    if (ctx->hm_known) return 0;
+    static const long long init[6] = {d2o(1e300), d2o(-1e300), d2o(1e300), d2o(-1e300), d2o(1e300), d2o(-1e300)};
+    CU(cudaMemcpyAsync(ctx->red, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
+    if (ctx->pool_end > 0) {
+        const unsigned nb = (unsigned)std::min<int64_t>(cdiv(ctx->pool_end, 256), REDUCE_BLOCKS);
+        k_reduce_minmax<<<nb, 256, 0, ctx->stream>>>(ctx->f64[B200SPH_H], ctx->f64[B200SPH_M], ctx->f64[B200SPH_M],
+                                                     nullptr, ctx->ptype, ctx->pool_end, 1, 0, ctx->red);
+        LAUNCH_CHECK();
+    }
+    CU(cudaMemcpyAsync(ctx->red_host, ctx->red, 4 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    const double h0 = o2d(ctx->red_host[0]), h1 = o2d(ctx->red_host[1]);
+    const double m0 = o2d(ctx->red_host[2]), m1 = o2d(ctx->red_host[3]);
+    ctx->h_uniform = (h0 == h1 && h0 > 0.0) ? h0 : NAN;
+    ctx->m_uniform = (m0 == m1) ? m0 : NAN;
+    ctx->hm_known = true;
+    return 0;
+}
+
 int b200sph_set_domain(b200sph_ctx *ctx, const double lo[3], const double hi[3], const int periodic[3])
 {
     if ((periodic[0] || periodic[1] || periodic[2]) && (ctx->mirror[0] || ctx->mirror[1] || ctx->mirror[2]))
@@ -1450,6 +1516,7 @@ static int nnps_light_update(b200sph_ctx *ctx)
         k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
             ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H], ctx->perm, ctx->skey,
             ctx->n_sorted, ctx->G, ctx->A0, ctx->A, ctx->AB, ctx->red_u32);
+        ctx->ab_stale = false;   // (k_pack_pos_light writes the position half of AB)
         LAUNCH_CHECK();
         return 1;
     }
@@ -1458,6 +1525,7 @@ static int nnps_light_update(b200sph_ctx *ctx)
         k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
             ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H], ctx->perm, ctx->skey,
             ctx->n_sorted, ctx->G, ctx->A0, ctx->A, ctx->AB, ctx->red_u32);
+        ctx->ab_stale = false;   // (k_pack_pos_light writes the position half of AB)
         LAUNCH_CHECK();
     }
     drift_consumed(ctx);
@@ -1716,6 +1784,7 @@ int b200sph_nnps_update(b200sph_ctx *ctx)
     }
     ctx->topo_dirty = false;
     ctx->grid_valid = true;
+    ctx->ab_stale = false;   // (k_pack_pos wrote AB)
     state_changed(ctx);   // new sorted slots
     return 0;
 }
@@ -1868,9 +1937,32 @@ static int eos_flush(b200sph_ctx *ctx, cudaStream_t on_comm_stream)
     return 0;
 }
 
+// Every reader of the position half of AB other than k_pair_list_r32 calls this first: after
+// k_stage_pack wrote the 32-byte records, the positions are in R only.
+static int ab_positions(b200sph_ctx *ctx)
+{
+    if (!ctx->ab_stale) return 0;
+    if (ctx->n_sorted > 0) {
+        k_rec32_positions<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(ctx->R, ctx->f64[B200SPH_H], ctx->perm,
+                                                                                       ctx->n_sorted, ctx->AB);
+        LAUNCH_CHECK();
+    }
+    ctx->ab_stale = false;
+    return 0;
+}
+
 static int pack_state(b200sph_ctx *ctx)
 {
-    if (ctx->n_sorted > 0) {
+    if (int rc = ab_positions(ctx)) return rc;   // (k_pack_rec32 reads them)
+    if (ctx->rec32 && ctx->n_sorted > 0) {
+        // (every particle is sorted: no ghosts, so the pool side of the EOS calls is complete)
+        k_pack_rec32<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
+            ctx->f64[B200SPH_U], ctx->f64[B200SPH_V], ctx->f64[B200SPH_W], ctx->f64[B200SPH_RHO], f32_ptr(ctx, B200SPH_P),
+            f32_ptr(ctx, B200SPH_CS), ctx->ptype, ctx->perm, ctx->n_sorted, ctx->AB, ctx->R, ctx->eos_pending, ctx->rec32_rho0);
+        LAUNCH_CHECK();
+        memset(ctx->eos_pending.on, 0, sizeof(ctx->eos_pending.on));
+        ctx->eos_any = false;
+    } else if (ctx->n_sorted > 0) {
         k_pack_state<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
             ctx->f64[B200SPH_U], ctx->f64[B200SPH_V], ctx->f64[B200SPH_W], ctx->f64[B200SPH_M], ctx->f64[B200SPH_RHO],
             f32_ptr(ctx, B200SPH_P), f32_ptr(ctx, B200SPH_CS), ctx->ptype, ctx->perm, ctx->n_sorted, ctx->B, ctx->C, ctx->AB,
@@ -1892,6 +1984,8 @@ int64_t b200sph_get_neighbors(b200sph_ctx *ctx, int dst_arr, int src_arr, int64_
     if (dst_arr < 0 || dst_arr >= ctx->narr || src_arr < 0 || src_arr >= ctx->narr) return set_err(ctx, "get_neighbors: bad array index");
     if (d_idx < 0 || d_idx >= ctx->arr[dst_arr].n) return set_err(ctx, "get_neighbors: d_idx out of range");
     int rc;
+    if (ctx->rec32) ctx->rec32 = false, state_changed(ctx);   // k_neighbors reads the 48-byte records
+    if ((rc = ab_positions(ctx))) return rc;
     if (!ctx->state_packed && (rc = pack_state(ctx))) return rc;
     uint32_t s32 = 0;
     CU(cudaMemcpyAsync(&s32, ctx->rank + ctx->arr[dst_arr].off + d_idx, 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2067,7 +2161,7 @@ int b200sph_generic_launch(b200sph_ctx *ctx, int module, const char *kernel, int
     if (dest_arr < 0 || dest_arr >= ctx->narr || phase < 0 || phase > 2) return set_err(ctx, "generic_launch: bad destination / phase");
     if (ctx->peer_box || ctx->comm_pending) return set_err(ctx, "generic equations run on one GPU (no slab decomposition)");
     if (!ctx->grid_valid) return set_err(ctx, "generic_launch: the NNPS is stale (particles were pushed/resized); call nnps_update first");
-    if ((rc = eos_flush(ctx))) return rc;
+    if ((rc = eos_flush(ctx)) || (rc = ab_positions(ctx))) return rc;
     const bool ranged = ctx->dst_ranged;   // one-shot, as for pair_pass: every launch names its own
     ctx->dst_ranged = false;
     static const char no_lists[] = "generic equations need the neighbour-list path";
@@ -2113,7 +2207,7 @@ int b200sph_generic_launch(b200sph_ctx *ctx, int module, const char *kernel, int
     }
     // what was derived from the properties the bodies stored to is stale
     if (writes & 1) h_changed(ctx);
-    if (writes & 2) state_changed(ctx), ctx->spec_records = false;
+    if (writes & 2) state_changed(ctx), m_changed(ctx), ctx->spec_records = false;
     return 0;
 }
 
@@ -2126,6 +2220,33 @@ int b200sph_set_dest_range(b200sph_ctx *ctx, int arr, int64_t start, int64_t sto
     ctx->dst_lo[arr] = start;
     ctx->dst_hi[arr] = stop;
     ctx->dst_ranged = true;
+    return 0;
+}
+
+// The 32-byte records (k_pair_list_r32) serve a list-walking pass of the WCSPH scheme's Group
+// (not ranged) when every array has a pending Tait EOS with gamma = 7 and the same rho0, c0
+// and pressure offset, h and m are the same for every particle, and there are no ghosts (the
+// slab halo and the mirror images write 48-byte records).  B200SPH_RECORDS=48 keeps the
+// 48-byte layout everywhere.
+static double eos_offset(const EosTab &E, int a) { return E.hg[a] ? 0.0 : E.p0[a]; }
+static int records32(b200sph_ctx *ctx, const bool wcsph_list_pass, bool *yes, int *eos_arr)
+{
+    *yes = false;
+    if (ctx->rec48_forced || !wcsph_list_pass || !ctx->eos_any || mirror_any(ctx) || ctx->peer_box || ctx->comm_pending)
+        return 0;
+    const EosTab &E = ctx->eos_pending;
+    int &first = *eos_arr;
+    first = -1;
+    for (int a = 0; a < ctx->narr; a++) {
+        if (ctx->arr[a].n != ctx->arr[a].n_real) return 0;
+        if (ctx->arr[a].n == 0) continue;
+        if (!E.on[a] || E.gamma[a] != 7.0) return 0;
+        if (first < 0) first = a;
+        else if (E.rho0[a] != E.rho0[first] || E.c0[a] != E.c0[first] || eos_offset(E, a) != eos_offset(E, first)) return 0;
+    }
+    if (first < 0) return 0;
+    if (int rc = hm_uniformity(ctx)) return rc;
+    *yes = !std::isnan(ctx->h_uniform) && !std::isnan(ctx->m_uniform);
     return 0;
 }
 
@@ -2159,6 +2280,22 @@ int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_
     ctx->dst_ranged = false;
     if (ranged && !use_lists && ctx->n_sorted > 0)
         return set_err(ctx, "pair_pass: destination ranges (Group start_idx / stop_idx) need the neighbour-list path");
+    // the WCSPH scheme's Group (continuity + momentum + XSPH, no tensile correction) has a
+    // leaner kernel variant, and may have 32-byte records
+    unsigned prog_bits = 0;
+    for (int d = 0; d < ctx->narr; d++)
+        for (int sx = 0; sx < ctx->narr; sx++) prog_bits |= prog->eqmask[d][sx];
+    const bool wcsph_only = !(prog_bits & ~(unsigned)PAIR_EQS_WCSPH) && !prog->tensile_correction;
+    bool r32 = false;
+    int ea = -1;
+    if ((rc = records32(ctx, use_lists && !ranged && wcsph_only, &r32, &ea))) return rc;
+    const EosTab E32 = ctx->eos_pending;   // (packing the state retires the pending calls)
+    if (r32 != ctx->rec32 || (r32 && E32.rho0[ea] != ctx->rec32_rho0)) {
+        ctx->rec32 = r32;
+        ctx->rec32_rho0 = r32 ? E32.rho0[ea] : 0.0;
+        state_changed(ctx);
+    }
+    if (!r32 && (rc = ab_positions(ctx))) return rc;
     // the (destination, source) type pairs this Group has equations for; lists that were
     // filtered with a narrower set are rebuilt with the union
     unsigned long long want[B200SPH_MAX_ARRAYS];
@@ -2215,12 +2352,16 @@ int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_
     pa.nu4 = (float)(4.0 * prog->nu); pa.eta = (float)prog->eta;
     pa.tensile = prog->tensile_correction;
     pa.real_only = prog->real_only;
-    // the WCSPH scheme's Group (continuity + momentum + XSPH, no tensile correction) has a
-    // leaner kernel variant
-    unsigned prog_bits = 0;
-    for (int d = 0; d < ctx->narr; d++)
-        for (int sx = 0; sx < ctx->narr; sx++) prog_bits |= prog->eqmask[d][sx];
-    const bool wcsph_only = !(prog_bits & ~(unsigned)PAIR_EQS_WCSPH) && !prog->tensile_correction;
+    if (r32) {
+        const double rho0 = E32.rho0[ea], c0 = E32.c0[ea];
+        pa.R = ctx->R;
+        pa.h = (float)ctx->h_uniform;        // the float every A record holds
+        pa.m = (float)ctx->m_uniform;
+        pa.rho0 = (float)rho0;
+        pa.eos_c0 = (float)c0;
+        pa.kB = (float)(c0 * c0 / (7.0 * rho0));   // B / rho0^2, B = rho0 c0^2 / gamma
+        pa.kp = (float)(eos_offset(E32, ea) / (rho0 * rho0));
+    }
     if (ranged)
         for (int d = 0; d < ctx->narr; d++) {
             pa.doff[d] = ctx->arr[d].off;
@@ -2246,7 +2387,8 @@ int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_
             if (nb == 0) continue;
             rc = with_kernel_dim(ctx, "pair_pass", [&](auto kc, auto dc) {
                 constexpr int K = decltype(kc)::value, D = decltype(dc)::value;
-                if (ranged) k_pair_list<K, D, 6, PAIR_EQS_ALL, true><<<nb, LIST_NT, 0, lst_stream>>>(pa, ctx->cnt, ctx->lst, ctx->capg, ids);
+                if (r32) k_pair_list_r32<K, D><<<nb, LIST_NT, 0, lst_stream>>>(pa, ctx->cnt, ctx->lst, ctx->capg);
+                else if (ranged) k_pair_list<K, D, 6, PAIR_EQS_ALL, true><<<nb, LIST_NT, 0, lst_stream>>>(pa, ctx->cnt, ctx->lst, ctx->capg, ids);
                 else if (wcsph_only) k_pair_list<K, D, 7, PAIR_EQS_WCSPH><<<nb, LIST_NT, 0, lst_stream>>>(pa, ctx->cnt, ctx->lst, ctx->capg, ids);
                 else k_pair_list<K, D, 7, PAIR_EQS_ALL><<<nb, LIST_NT, 0, lst_stream>>>(pa, ctx->cnt, ctx->lst, ctx->capg, ids);
                 LAUNCH_CHECK();
@@ -2267,6 +2409,7 @@ int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_
             }
         }
         ctx->stats.pair_launches++;
+        if (r32) ctx->n_pair_r32++;
     } else if (ctx->n_sorted > 0) {
         const unsigned nb = (unsigned)cdiv(ctx->n_sorted, PAIR_WARPS * PAIR_CHUNK);
         rc = with_kernel_dim(ctx, "pair_pass", [&](auto kc, auto dc) {
@@ -2307,6 +2450,7 @@ int b200sph_tvf_pass(b200sph_ctx *ctx, const b200sph_tvf_program *prog, int64_t 
         return set_err(ctx, "tvf_pass: with solid walls the average pressure is computed after the wall pressure (passes bit 2), not in group 1");
     if (solid_mask && (ctx->peer_box || ctx->comm_pending)) return set_err(ctx, "tvf_pass: EDAC with solid walls runs on one GPU");
     if (ctx->n_sorted == 0) return 0;
+    if ((rc = ab_positions(ctx))) return rc;
     // (these passes take unfiltered lists)
     if ((rc = prepare_lists(ctx, nullptr, "tvf_pass: the EDAC kernels need the neighbour-list path (B200SPH_PAIR_KERNEL=list, < 2^26 particles)")))
         return rc;
@@ -2394,6 +2538,7 @@ int b200sph_solid_pass(b200sph_ctx *ctx, const b200sph_solid_program *prog, int6
     if (!(prog->passes & 3)) return set_err(ctx, "solid_pass: passes must select group 1 and/or group 2");
     if (prog->elastic_mask == 0 || prog->elastic_mask >= (1u << ctx->narr)) return set_err(ctx, "solid_pass: bad elastic mask 0x%x", prog->elastic_mask);
     if (ctx->n_sorted == 0) return 0;
+    if ((rc = ab_positions(ctx))) return rc;
     // (these passes take unfiltered lists)
     if ((rc = prepare_lists(ctx, nullptr, "solid_pass: the elastic-dynamics kernels need the neighbour-list path"))) return rc;
     SolidArgs sa;
@@ -2557,6 +2702,8 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
         q.p = f32_ptr(ctx, B200SPH_P); q.cs = f32_ptr(ctx, B200SPH_CS);
         q.rank = ctx->rank; q.key_of = ctx->key_of;
         q.A0 = ctx->A0; q.AB = ctx->AB; q.C = ctx->C;
+        q.R = ctx->rec32 ? ctx->R : nullptr;   // the layout the last pair pass read
+        q.rho0 = ctx->rec32_rho0;
         q.G = ctx->G;
         q.red_u32 = ctx->red_u32;
         q.dt_cfl = f32_ptr(ctx, B200SPH_DT_CFL); q.dt_force = f32_ptr(ctx, B200SPH_DT_FORCE);
@@ -2578,6 +2725,7 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
         if (which == 2) ctx->dt_reduced = q.reduce_dt != 0, ctx->dt_adaptive_seen = false;
         positions_changed(ctx);        // particles moved: nnps_update must decide about the lists
         ctx->packed_valid = true;      // ... but their packed positions are current,
+        ctx->ab_stale = q.R != nullptr;    // (in R only, with the 32-byte records)
         ctx->drift_measured = true;    // the drift of the build is in red_u32,
         ctx->state_packed = true;      // and so is their packed state,
         ctx->spec_records = ctx->eos_last_valid;   // with last evaluation's EOS calls applied
@@ -3007,6 +3155,7 @@ int b200sph_nnps_drift(b200sph_ctx *ctx, double out[2])
         k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
             ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H], ctx->perm, ctx->skey,
             ctx->n_sorted, ctx->G, ctx->A0, ctx->A, ctx->AB, ctx->red_u32);
+        ctx->ab_stale = false;   // (k_pack_pos_light writes the position half of AB)
         LAUNCH_CHECK();
     }
     CU(cudaMemcpyAsync(ctx->red_u32_host, ctx->red_u32, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
@@ -3135,6 +3284,7 @@ int b200sph_nnps_drift_device(b200sph_ctx *ctx, double *dev_ratio)
         k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
             ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H], ctx->perm, ctx->skey,
             ctx->n_sorted, ctx->G, ctx->A0, ctx->A, ctx->AB, ctx->red_u32);
+        ctx->ab_stale = false;   // (k_pack_pos_light writes the position half of AB)
         LAUNCH_CHECK();
     }
     k_drift_ratio<<<1, 1, 0, ctx->stream>>>(ctx->red_u32, (float)ctx->radius_scale, (float)ctx->S_abs, dev_ratio);
@@ -3249,6 +3399,7 @@ int b200sph_peer_begin(b200sph_ctx *ctx)
         k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
             ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H], ctx->perm, ctx->skey,
             ctx->n_sorted, ctx->G, ctx->A0, ctx->A, ctx->AB, ctx->red_u32);
+        ctx->ab_stale = false;   // (k_pack_pos_light writes the position half of AB)
         LAUNCH_CHECK();
     }
     if (!no_build) ctx->packed_valid = true, ctx->drift_measured = true;
@@ -3668,7 +3819,12 @@ int b200sph_reset_stats(b200sph_ctx *ctx)
     b200sph_stats tmp;
     b200sph_get_stats(ctx, &tmp);  // drain pending events
     memset(&ctx->stats, 0, sizeof(ctx->stats));
-    ctx->n_full_builds = ctx->n_light_updates = ctx->n_list_builds = ctx->n_deferred_failed = ctx->n_fused = ctx->n_overlapped = ctx->n_proactive = 0;
+    ctx->n_full_builds = ctx->n_light_updates = ctx->n_list_builds = ctx->n_deferred_failed = ctx->n_fused = ctx->n_overlapped = ctx->n_proactive = ctx->n_pair_r32 = 0;
+    return 0;
+}
+int b200sph_records32_launches(b200sph_ctx *ctx, int64_t *out)
+{
+    *out = ctx->n_pair_r32;
     return 0;
 }
 int b200sph_set_async_copies(b200sph_ctx *ctx, int on)

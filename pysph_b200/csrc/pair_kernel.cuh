@@ -25,6 +25,11 @@ struct PairArgs {
     // Group(start_idx, stop_idx): destinations [dlo, dhi) of every array, as indices INTO the
     // array (equation.py:448-520); read by the RANGED instantiations of k_pair_list only
     long long doff[B200SPH_MAX_ARRAYS], dlo[B200SPH_MAX_ARRAYS], dhi[B200SPH_MAX_ARRAYS];
+    // k_pair_list_r32 only: the 32-byte records, the uniform h and m, and the one Tait EOS
+    // (gamma = 7) of every array: rho = rho0 (1 + delta), cs = eos_c0 (1 + delta)^3,
+    // p / rho^2 = (kB ((1 + delta)^7 - 1) + kp) / (1 + delta)^2 with kB = B / rho0^2, kp = p0 / rho0^2
+    const float4 *R;
+    float h, m, rho0, eos_c0, kB, kp;
 };
 
 #define PAIR_WARPS 8

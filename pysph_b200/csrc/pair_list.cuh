@@ -251,11 +251,10 @@ __device__ __forceinline__ float4 list_cell_offset(const uint32_t e, const float
 // one list entry: cell-offset lookup, distance, the exact accept test, the equations.  `live`
 // is false for the lanes whose list is shorter than the warp's longest (their entry reads
 // as 0 and their record as record 0, so everything up to the test is harmless to execute).
-template <int K, int DIM, int EQS>
-__device__ __forceinline__ void pair_entry(const PairArgs &a, const bool live, const uint32_t e,
-                                           const float4 Aj, const float4 Bj, const float4 Cj, const float4 Ai,
-                                           const float4 Bi, const float4 Ci, const float hi2,
-                                           const unsigned long long mask_i, Acc &acc, unsigned &npairs)
+// x_ij of a list entry and its square; both list consumers of the WCSPH Group use this one
+// expression, so that they take the same accept decisions on the same positions
+__device__ __forceinline__ float entry_dist(const PairArgs &a, const uint32_t e, const float4 Ai, const float4 Aj,
+                                            float &xij, float &yij, float &zij)
 {
     // cell offset of the neighbour's cell relative to the destination's, decoded arithmetically:
     // (code field | 0x4B000000) as a float is 2^23 + field, exactly, so field - 1 costs one
@@ -264,9 +263,19 @@ __device__ __forceinline__ void pair_entry(const PairArgs &a, const bool live, c
     const float dxc = __uint_as_float((e & 3u) | 0x4B000000u) - 8388609.0f;
     const float dyc = __uint_as_float(((e >> 2) & 3u) | 0x4B000000u) - 8388609.0f;
     const float dzc = __uint_as_float(((e >> 4) & 3u) | 0x4B000000u) - 8388609.0f;
-    const float xij = fmaf(-dxc, a.cellx, Ai.x - Aj.x), yij = fmaf(-dyc, a.celly, Ai.y - Aj.y),
-                zij = fmaf(-dzc, a.cellz, Ai.z - Aj.z);
-    const float r2 = xij * xij + yij * yij + zij * zij;
+    xij = fmaf(-dxc, a.cellx, Ai.x - Aj.x), yij = fmaf(-dyc, a.celly, Ai.y - Aj.y),
+    zij = fmaf(-dzc, a.cellz, Ai.z - Aj.z);
+    return xij * xij + yij * yij + zij * zij;
+}
+
+template <int K, int DIM, int EQS>
+__device__ __forceinline__ void pair_entry(const PairArgs &a, const bool live, const uint32_t e,
+                                           const float4 Aj, const float4 Bj, const float4 Cj, const float4 Ai,
+                                           const float4 Bi, const float4 Ci, const float hi2,
+                                           const unsigned long long mask_i, Acc &acc, unsigned &npairs)
+{
+    float xij, yij, zij;
+    const float r2 = entry_dist(a, e, Ai, Aj, xij, yij, zij);
     // the exact accept test, linked_list_nnps.pyx:188
     if (live && ((r2 < hi2) || (r2 < a.k2 * Aj.w * Aj.w)))
         pair_body<K, DIM, EQS>(a, make_float4(xij, yij, zij, Aj.w), Bj, Cj, Ai, Bi, Ci, mask_i, Ci.y, acc, npairs);
@@ -332,6 +341,121 @@ __global__ void __launch_bounds__(LIST_NT, MINB) k_pair_list(const PairArgs a, c
         if (all_bits & B200SPH_EQ_XSPH) {
             // post_loop basic_equations.py:297-300
             a.ax[g] = acc.ax + Bi.x; a.ay[g] = acc.ay + Bi.y; a.az[g] = acc.az + Bi.z;
+        }
+    }
+    if (a.pair_counter) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) npairs += __shfl_xor_sync(FULL, npairs, o);
+        if ((tid & 31) == 0 && npairs) atomicAdd(a.pair_counter, (unsigned long long)npairs);
+    }
+}
+
+// (1 + d)^7 - 1 of the Tait EOS (gamma = 7) in Horner form: no cancellation for small d
+__device__ __forceinline__ float tait_p7(const float d)
+{
+    return d * fmaf(d, fmaf(d, fmaf(d, fmaf(d, fmaf(d, d + 7.0f, 21.0f), 35.0f), 35.0f), 21.0f), 7.0f);
+}
+
+// The list consumer of the 32-byte records (records32 in b200sph.cu: the WCSPH scheme's Group
+// with uniform h and m, one Tait EOS with gamma = 7 for every array, no ghosts).  Per entry ONE
+// ld_256 -- a single sector, two 128-bit loads where k_pair_list issues three into two sectors --
+// and what the 48-byte C record carried is recomputed from delta = rho / rho0 - 1: rho, cs and
+// p / rho^2 (one rcp).  h is uniform, so h_ij, 1 / h_ij and the kernel's normalisation are
+// per-thread constants, and the accept test is k_pair_list's on the same floats (the same
+// pairs); m is factored out of the sums.
+template <int K, int DIM>
+__global__ void __launch_bounds__(LIST_NT, 8) k_pair_list_r32(const PairArgs a, const uint32_t *__restrict__ cnt,
+                                                             const uint32_t *__restrict__ lst, const int capg)
+{
+    const int tid = threadIdx.x;
+    const unsigned FULL = 0xffffffffu;
+    const long long s = (long long)blockIdx.x * LIST_NT + tid;
+    bool active = s < a.n;
+    float4 Pi = make_float4(0.f, 0.f, 0.f, 0.f), Vi = Pi;
+    unsigned long long mask_i = 0;
+    int count = 0;
+    if (active) {
+        ld_256(a.R + 2 * (size_t)s, Pi, Vi);
+        const int ti = __float_as_int(Vi.w);
+        mask_i = a.emask[ti & 7];
+        if ((a.real_only && (ti & PT_GHOST)) || !mask_i) active = false;
+    }
+    if (active) count = (int)cnt[s];
+    int cmax = count;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) cmax = max(cmax, __shfl_xor_sync(FULL, cmax, o));
+    const uint32_t *nxt = lst + ((size_t)(s >> 5) * (size_t)capg) * 32u + (uint32_t)(s & 31);
+    const float h = a.h;
+    const float h2k = a.k2 * h * h;              // k_pair_list's hi2 (and hj2) on the same floats
+    const float h1 = frcp(h);
+    const float fac = a.kfac * hpow<DIM>(h1);
+    const float eta2 = 0.01f * h * h;
+    const float hrho0 = 0.5f * a.rho0;
+    const float xi = 1.0f + Pi.w, ixi = frcp(xi);
+    const float tmpi = fmaf(a.kB, tait_p7(Pi.w), a.kp) * (ixi * ixi);   // p_i / rho_i^2
+    const float csi = a.eos_c0 * (xi * xi * xi);
+    Acc acc = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    unsigned npairs = 0;
+    struct Rec { float4 P, V; };
+    list_walk<Rec>(nxt, count, cmax,
+        [&](const uint32_t e, Rec &r) { ld_256(a.R + 2u * LIST_J(e), r.P, r.V); },
+        [&](const bool live, const uint32_t e, const Rec &r) {
+            float xij, yij, zij;
+            const float r2 = entry_dist(a, e, Pi, r.P, xij, yij, zij);
+            if (!live || !(r2 < h2k)) return;    // the exact accept test, linked_list_nnps.pyx:188
+            const unsigned bits = (unsigned)(mask_i >> (8 * (__float_as_int(r.V.w) & 7))) & (unsigned)PAIR_EQS_WCSPH;
+            if (!bits) return;
+            npairs++;
+            // pair_body with h_j = h_i = h and m_j = m
+            const bool far = r2 > 1e-24f;
+            const float rinv = far ? frsqrt(r2) : 0.0f;
+            const float q = r2 * rinv * h1;
+            float w, dw;
+            sph_kernel<K>(q, w, dw);
+            const float gt = dw * fac * h1 * rinv;
+            const float uij = Vi.x - r.V.x, vij = Vi.y - r.V.y, wwij = Vi.z - r.V.z;
+            const float vdotx = uij * xij + vij * yij + wwij * zij;
+            if (bits & B200SPH_EQ_CONTINUITY) acc.arho += gt * vdotx;
+            if (bits & (B200SPH_EQ_MOMENTUM | B200SPH_EQ_XSPH)) {
+                const float dj = r.P.w;
+                const float rhoij1 = frcp(fmaf(hrho0, Pi.w + dj, a.rho0));
+                if (bits & B200SPH_EQ_MOMENTUM) {
+                    const float xj = 1.0f + dj, ixj = frcp(xj);
+                    const float cij = 0.5f * (csi + a.eos_c0 * (xj * xj * xj));
+                    const float muij = h * vdotx * frcp(r2 + eta2);
+                    const float piij = vdotx < 0.0f ? (-a.alpha * cij * muij + a.beta * muij * muij) * rhoij1 : 0.0f;
+                    if (r2 > 1e-12f) acc.cfl = fmaxf(acc.cfl, fabsf(h * vdotx * rinv * rinv) + a.c0);
+                    const float tmpj = fmaf(a.kB, tait_p7(dj), a.kp) * (ixj * ixj);
+                    const float f = (tmpi + tmpj + piij) * gt;    // times -m below
+                    acc.au += f * xij;
+                    acc.av += f * yij;
+                    acc.aw += f * zij;
+                }
+                if (bits & B200SPH_EQ_XSPH) {
+                    const float f = w * fac * rhoij1;              // times -eps m below
+                    acc.ax += f * uij;
+                    acc.ay += f * vij;
+                    acc.az += f * wwij;
+                }
+            }
+        });
+    if (active) {
+        unsigned all_bits = 0;
+#pragma unroll
+        for (int j = 0; j < B200SPH_MAX_ARRAYS; j++) all_bits |= (unsigned)(mask_i >> (8 * j)) & (unsigned)PAIR_EQS_WCSPH;
+        const uint32_t g = a.perm[s];
+        if (all_bits & B200SPH_EQ_CONTINUITY) a.arho[g] = a.m * acc.arho;
+        if (all_bits & B200SPH_EQ_MOMENTUM) {
+            // post_loop wc/basic.py:259-269
+            const float fu = fmaf(-a.m, acc.au, a.gx), fv = fmaf(-a.m, acc.av, a.gy), fw = fmaf(-a.m, acc.aw, a.gz);
+            a.au[g] = fu; a.av[g] = fv; a.aw[g] = fw;
+            a.dt_cfl[g] = acc.cfl;
+            a.dt_force[g] = fu * fu + fv * fv + fw * fw;
+        }
+        if (all_bits & B200SPH_EQ_XSPH) {
+            // post_loop basic_equations.py:297-300
+            const float me = -a.eps_xsph * a.m;
+            a.ax[g] = fmaf(me, acc.ax, Vi.x); a.ay[g] = fmaf(me, acc.ay, Vi.y); a.az[g] = fmaf(me, acc.az, Vi.z);
         }
     }
     if (a.pair_counter) {

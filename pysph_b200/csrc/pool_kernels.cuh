@@ -202,6 +202,8 @@ struct FusePackArgs {
     const uint32_t *rank, *key_of;   // pool index -> sorted slot / cell key of the current build
     const float4 *A0;                // packed positions at build time (sorted order)
     float4 *AB, *C;
+    float4 *R;                       // non-null: the state goes into the 32-byte records (rho0: of delta)
+    double rho0;
     GridDev G;
     unsigned *red_u32;
     const float *dt_cfl, *dt_force;
@@ -263,28 +265,37 @@ __global__ void __launch_bounds__(256, 5) k_stage_pack(const StageArgs a, const 
             A.y = (float)(yn - (q.G.xmin[1] + (double)cy * q.G.cell[1]));
             A.z = (float)(zn - (q.G.xmin[2] + (double)cz * q.G.cell[2]));
             A.w = (float)hg;
-            B.x = (float)un; B.y = (float)vn; B.z = (float)wn; B.w = (float)q.m[g];
-            float pg, csg;
             const int ar = t & 7;
-            if (q.eos_any && q.E.on[ar]) {   // real particle: real_only does not matter here
-                const double rho0 = q.E.rho0[ar];
-                if (q.E.hg[ar] && r < rho0) r = rho0;   // the record only: the pool keeps rho
-                const double ratio = r * (1.0 / rho0);
-                const double Bc = rho0 * q.E.c0[ar] * q.E.c0[ar] / q.E.gamma[ar];
-{ double rg_, rh_; tait_powers(ratio, q.E.gamma[ar], rg_, rh_);
-                pg = (float)((q.E.hg[ar] ? 0.0 : q.E.p0[ar]) + Bc * (rg_ - 1.0));
-                csg = (float)(q.E.c0[ar] * rh_); }
+            if (q.R) {
+                // only the full sector: a lone 16-byte half would cost a read-modify-write in
+                // HBM per particle (the position half of AB is restored from R on demand, ab_positions)
+                float4 R0, R1;
+                rec32_make(A, un, vn, wn, r, q.eos_any && q.E.on[ar] && q.E.hg[ar], q.rho0, (int)t, R0, R1);
+                q.R[2 * (size_t)s] = R0;
+                q.R[2 * (size_t)s + 1] = R1;
             } else {
-                pg = q.p[g];
-                csg = q.cs[g];
+                B.x = (float)un; B.y = (float)vn; B.z = (float)wn; B.w = (float)q.m[g];
+                float pg, csg;
+                if (q.eos_any && q.E.on[ar]) {   // real particle: real_only does not matter here
+                    const double rho0 = q.E.rho0[ar];
+                    if (q.E.hg[ar] && r < rho0) r = rho0;   // the record only: the pool keeps rho
+                    const double ratio = r * (1.0 / rho0);
+                    const double Bc = rho0 * q.E.c0[ar] * q.E.c0[ar] / q.E.gamma[ar];
+{ double rg_, rh_; tait_powers(ratio, q.E.gamma[ar], rg_, rh_);
+                    pg = (float)((q.E.hg[ar] ? 0.0 : q.E.p0[ar]) + Bc * (rg_ - 1.0));
+                    csg = (float)(q.E.c0[ar] * rh_); }
+                } else {
+                    pg = q.p[g];
+                    csg = q.cs[g];
+                }
+                C.x = (float)r;
+                C.y = (float)((double)pg / (r * r));
+                C.z = csg;
+                C.w = __int_as_float((int)t);
+                q.AB[2 * (size_t)s] = A;
+                q.AB[2 * (size_t)s + 1] = B;
+                q.C[s] = C;
             }
-            C.x = (float)r;
-            C.y = (float)((double)pg / (r * r));
-            C.z = csg;
-            C.w = __int_as_float((int)t);
-            q.AB[2 * (size_t)s] = A;
-            q.AB[2 * (size_t)s + 1] = B;
-            q.C[s] = C;
             const float4 b0 = q.A0[s];
             const float ex = A.x - b0.x, ey = A.y - b0.y, ez = A.z - b0.z;
             d2 = ex * ex + ey * ey + ez * ez;
@@ -331,13 +342,9 @@ __global__ void __launch_bounds__(256, 5) k_stage_pack(const StageArgs a, const 
 // TaitEOS.loop wc/basic.py:60-65 ; TaitEOSHGCorrection.loop wc/basic.py:118-126: the pending
 // equation-of-state calls of every array in one launch (pool side: rho clamp of the HG
 // variant, p, cs); same arithmetic as k_pack_state
-__global__ void k_eos_tab(double *__restrict__ rho, float *__restrict__ p, float *__restrict__ cs,
-                          const uint8_t *__restrict__ ptype, long long pool_end, const EosTab E)
+__device__ __forceinline__ void eos_tab_apply(double *__restrict__ rho, float *__restrict__ p, float *__restrict__ cs,
+                                              const uint8_t t, const long long g, const EosTab &E)
 {
-    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= pool_end) return;
-    const uint8_t t = ptype[g];
-    if (t == PT_INVALID) return;
     const int a = t & 7;
     if (!E.on[a] || (E.real_only[a] && (t & PT_GHOST))) return;
     double r = rho[g];
@@ -351,6 +358,46 @@ __global__ void k_eos_tab(double *__restrict__ rho, float *__restrict__ p, float
 { double rg_, rh_; tait_powers(ratio, E.gamma[a], rg_, rh_);
     p[g] = (float)((E.hg[a] ? 0.0 : E.p0[a]) + Bc * (rg_ - 1.0));
     cs[g] = (float)(E.c0[a] * rh_); }
+}
+__global__ void k_eos_tab(double *__restrict__ rho, float *__restrict__ p, float *__restrict__ cs,
+                          const uint8_t *__restrict__ ptype, long long pool_end, const EosTab E)
+{
+    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= pool_end) return;
+    const uint8_t t = ptype[g];
+    if (t == PT_INVALID) return;
+    eos_tab_apply(rho, p, cs, t, g, E);
+}
+
+// R[s] = the 32-byte records (rec32_make) from the packed positions (the position half of AB)
+// and the pool's state, with the pending EOS calls applied to the pool on the way (k_eos_tab's
+// arithmetic; in the record they only decide the clamp of TaitEOSHGCorrection)
+__global__ void k_pack_rec32(const double *__restrict__ u, const double *__restrict__ v,
+                             const double *__restrict__ w, double *__restrict__ rho, float *__restrict__ p,
+                             float *__restrict__ cs, const uint8_t *__restrict__ ptype,
+                             const uint32_t *__restrict__ perm, long long n, const float4 *__restrict__ AB,
+                             float4 *__restrict__ R, const EosTab E, const double rho0)
+{
+    long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    const uint32_t g = perm[s];
+    const uint8_t t = ptype[g];
+    eos_tab_apply(rho, p, cs, t, g, E);
+    float4 R0, R1;
+    rec32_make(AB[2 * s], u[g], v[g], w[g], rho[g], E.on[t & 7] && E.hg[t & 7], rho0, (int)t, R0, R1);
+    R[2 * s] = R0;
+    R[2 * s + 1] = R1;
+}
+
+// the position half of AB from the 32-byte records (after k_stage_pack wrote only R):
+// the same floats k_pack_pos_light computes, for the readers of the 48-byte records
+__global__ void k_rec32_positions(const float4 *__restrict__ R, const double *__restrict__ h,
+                                  const uint32_t *__restrict__ perm, long long n, float4 *__restrict__ AB)
+{
+    long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    const float4 r = R[2 * s];
+    AB[2 * s] = make_float4(r.x, r.y, r.z, (float)h[perm[s]]);
 }
 
 // k_dt_propose + k_dt_commit in one launch (one rank: nothing to reduce in between), and
