@@ -111,7 +111,8 @@ def test_sph_evaluator_periodic_fixture(gpu_device):
     assert dest.rho[0] < 7.5
 
 
-def _periodic_case(dim, n, seed=3):
+def _periodic_case(dim, n, seed=3, tensile=True):
+    """tensile=False runs the pair pass on the 32-byte records; beta != 0 then"""
     import pysph_b200 as pb
     pa, dx = _lattice(dim, n, hdx=1.3)
     rs = np.random.RandomState(seed)
@@ -127,19 +128,30 @@ def _periodic_case(dim, n, seed=3):
     pa.rho[:] = rho0 * (1 + 0.01 * rs.uniform(-1, 1, pa.x.size))
     pa.m[:] = rho0 * dx ** dim
     params = dict(fluids=['fluid'], solids=[], dim=dim, rho0=rho0, c0=10.0,
-                  h0=1.3 * dx, hdx=1.3, gamma=7.0, alpha=0.1, beta=0.0,
-                  tensile_correction=True, dt0=1e-4, cfl=0.3, integrator='EPEC')
+                  h0=1.3 * dx, hdx=1.3, gamma=7.0, alpha=0.1, beta=0.0 if tensile else 0.3,
+                  tensile_correction=tensile, dt0=1e-4, cfl=0.3, integrator='EPEC')
     return pa, params
 
 
-@pytest.mark.parametrize('dim,n,pattern', [(2, 24, (1, 1, 0)), (3, 10, (1, 1, 1)),
-                                           (3, 10, (1, 0, 1)), (2, 24, (0, 1, 0))])
-def test_periodic_wcsph_steps_vs_oracle(gpu_device, dim, n, pattern):
+@pytest.mark.parametrize('dim,n,pattern,tensile', [
+    pytest.param(2, 24, (1, 1, 0), True, id='2-24-pattern0'),
+    pytest.param(3, 10, (1, 1, 1), True, id='3-10-pattern1'),
+    pytest.param(3, 10, (1, 0, 1), True, id='3-10-pattern2'),
+    pytest.param(2, 24, (0, 1, 0), True, id='2-24-pattern3'),
+    pytest.param(2, 24, (1, 1, 0), False, id='2-24-pattern0-no_tensile'),
+    pytest.param(3, 10, (1, 0, 1), False, id='3-10-pattern2-no_tensile')])
+def test_periodic_wcsph_steps_vs_oracle(gpu_device, dim, n, pattern, tensile):
+    periodic_wcsph_steps_vs_oracle(gpu_device, dim, n, pattern, tensile)
+
+
+# (test_library_on_cpu.py runs this on the library emulation; tensile is on unless it says not)
+def periodic_wcsph_steps_vs_oracle(gpu_device, dim, n, pattern, tensile=True):
     """5 EPEC steps (continuity + momentum + AV + tensile + XSPH + Tait) in a
-    box periodic along `pattern`, against the ghost-materialising oracle."""
+    box periodic along `pattern`, against the ghost-materialising oracle.  Without
+    the tensile correction every pair pass takes the 32-byte records."""
     import pysph_b200 as pb
-    pa, params = _periodic_case(dim, n)
-    ref_pa, _ = _periodic_case(dim, n)
+    pa, params = _periodic_case(dim, n, tensile=tensile)
+    ref_pa, _ = _periodic_case(dim, n, tensile=tensile)
     dm = pb.DomainManager(xmin=0, xmax=1, ymin=0, ymax=1, zmin=0,
                           zmax=1 if dim == 3 else 0,
                           periodic_in_x=bool(pattern[0]),
@@ -173,6 +185,9 @@ def test_periodic_wcsph_steps_vs_oracle(gpu_device, dim, n, pattern):
         scale = max(np.max(np.abs(ref)), 1e-12)
         assert np.max(np.abs(pa.properties[k][order] - ref)) <= 2e-5 * scale, k
     assert abs(s.t - o.t) <= 1e-6 * o.t
+    if not tensile:
+        st = s.backend.stats()
+        assert st['pair_launches_r32'] == st['pair_launches'] > 0, st
 
 
 def test_periodic_translation_invariance_and_momentum(gpu_device):
