@@ -139,18 +139,15 @@ __host__ __device__ static inline void tait_powers(const double ratio, const dou
     }
 }
 
-// The 32-byte record of the WCSPH pass when h, m and the Tait EOS (gamma = 7) are the same for
-// every particle (records32 in b200sph.cu): R = {(x, y, z, delta), (u, v, w, type)} with
-// delta = rho / rho0 - 1 formed in fp64 after the clamp of TaitEOSHGCorrection, so that fp32
-// keeps the digits of the density variation; k_pair_list_r32 recomputes rho, p / rho^2 and cs
-// from delta.  ONE function for every writer, so that they all produce the same bits.
-__device__ __forceinline__ void rec32_make(const float4 A, const double u, const double v, const double w, double rho,
-                                           const bool clamp, const double rho0, const int type, float4 &R0, float4 &R1)
-{
-    if (clamp && rho < rho0) rho = rho0;
-    R0 = make_float4(A.x, A.y, A.z, (float)(rho * (1.0 / rho0) - 1.0));
-    R1 = make_float4((float)u, (float)v, (float)w, __int_as_float(type));
-}
+// The one Tait EOS (gamma = 7) the 32-byte records are formed with: rho0, B = rho0 c0^2 / 7 and
+// the pressure offset (p0 of TaitEOS, 0 with TaitEOSHGCorrection).  The records depend on these
+// three values only, so they are also the key that says when the records must be repacked.
+struct Rec32Eos {
+    double rho0, B, poff;
+    // folded on the host for rec32_make: kB (1, 7, 21, 35) with kB = B / rho0^2, and poff / rho0^2
+    float tait[4], kp;
+    bool operator!=(const Rec32Eos &o) const { return rho0 != o.rho0 || B != o.B || poff != o.poff; }
+};
 
 struct PendingEvent {
     cudaEvent_t e0, e1;
@@ -220,11 +217,11 @@ struct b200sph_ctx {
     uint32_t *perm_tmp = nullptr, *perm = nullptr, *skey = nullptr, *rank = nullptr;
     float4 *A = nullptr, *B = nullptr, *C = nullptr;
     float4 *AB = nullptr;  // {A, B} interleaved (32 B = one sector per particle) for the list consumer's 256-bit gathers
-    // the 32-byte records of the WCSPH pass (records32): {(x, y, z, rho / rho0 - 1), (u, v, w, type)};
+    // the 32-byte records of the WCSPH pass (records32): {(x, y, z, p / rho^2), (u, v, w, delta + type)};
     // while rec32 holds, the state records are packed HERE instead of B / C / the B half of AB
     float4 *R = nullptr;
     bool rec32 = false;
-    double rec32_rho0 = 0.0;    // the rho0 of the packed delta
+    Rec32Eos rec32_eos = {};    // the EOS the records are packed with
     bool ab_stale = false;      // k_stage_pack wrote the positions into R only (ab_positions restores AB)
     bool rec48_forced = false;  // env B200SPH_RECORDS=48
     // h and m over all particles (records32 needs both uniform): computed on demand by one
@@ -549,6 +546,29 @@ __device__ __forceinline__ unsigned long long peer_now_ns()
 #endif
 
 #include "generic_args.h"
+// The 32-byte record of the WCSPH pass when h, m and the Tait EOS (gamma = 7) are the same for
+// every particle (records32 in b200sph.cu): R = {(x, y, z, tau), (u, v, w, delta')} with
+//   delta = rho / rho0 - 1 formed in fp64 after the clamp of TaitEOSHGCorrection, so that fp32
+//     keeps the digits of the density variation;
+//   tau = p / rho^2 = (kB ((1 + delta)^7 - 1) + kp) / (1 + delta)^2, the source's pressure term,
+//     from delta in fp32 (the Tait polynomial in Horner form: no cancellation for small delta)
+//     -- the arithmetic k_pair_list_r32 used to repeat for every pair, so the same bits;
+//   delta' = delta with the array type (0..7; no ghosts on this path) in its 3 low mantissa bits.
+//     That moves delta by at most 7 ulp, ~1e-9 rho0 at |delta| <= 0.02, far below the fp32
+//     rounding of rho; k_pair_list_r32 takes rho and cs from delta' as it is, the type from its
+//     low bits.
+// ONE function for every writer, so that they all produce the same bits.
+__device__ __forceinline__ void rec32_make(const float4 A, const double u, const double v, const double w, double rho,
+                                           const bool clamp, const Rec32Eos &E, const int type, float4 &R0, float4 &R1)
+{
+    if (clamp && rho < E.rho0) rho = E.rho0;
+    const float d = (float)(rho * (1.0 / E.rho0) - 1.0);
+    const float x = 1.0f + d;
+    const float t = fmaf(fmaf(fmaf(fmaf(fmaf(d, E.tait[0], E.tait[1]), d, E.tait[2]), d, E.tait[3]), d, E.tait[3]), d, E.tait[2]);
+    R0 = make_float4(A.x, A.y, A.z, fmaf(fmaf(t, d, E.tait[1]), d, E.kp) * frcp(x * x));
+    R1 = make_float4((float)u, (float)v, (float)w, __int_as_float((__float_as_int(d) & ~7) | (type & 7)));
+}
+
 #include "pool_kernels.cuh"
 #include "scan.cuh"
 #include "nnps_kernels.cuh"
@@ -1958,7 +1978,7 @@ static int pack_state(b200sph_ctx *ctx)
         // (every particle is sorted: no ghosts, so the pool side of the EOS calls is complete)
         k_pack_rec32<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
             ctx->f64[B200SPH_U], ctx->f64[B200SPH_V], ctx->f64[B200SPH_W], ctx->f64[B200SPH_RHO], f32_ptr(ctx, B200SPH_P),
-            f32_ptr(ctx, B200SPH_CS), ctx->ptype, ctx->perm, ctx->n_sorted, ctx->AB, ctx->R, ctx->eos_pending, ctx->rec32_rho0);
+            f32_ptr(ctx, B200SPH_CS), ctx->ptype, ctx->perm, ctx->n_sorted, ctx->AB, ctx->R, ctx->eos_pending, ctx->rec32_eos);
         LAUNCH_CHECK();
         memset(ctx->eos_pending.on, 0, sizeof(ctx->eos_pending.on));
         ctx->eos_any = false;
@@ -2229,6 +2249,12 @@ int b200sph_set_dest_range(b200sph_ctx *ctx, int arr, int64_t start, int64_t sto
 // slab halo and the mirror images write 48-byte records).  B200SPH_RECORDS=48 keeps the
 // 48-byte layout everywhere.
 static double eos_offset(const EosTab &E, int a) { return E.hg[a] ? 0.0 : E.p0[a]; }
+static Rec32Eos rec32_eos(const EosTab &E, int a)
+{
+    const double rho0 = E.rho0[a], B = rho0 * E.c0[a] * E.c0[a] / 7.0, kB = B / (rho0 * rho0);
+    return Rec32Eos{rho0, B, eos_offset(E, a), {(float)kB, (float)(7.0 * kB), (float)(21.0 * kB), (float)(35.0 * kB)},
+                    (float)(eos_offset(E, a) / (rho0 * rho0))};
+}
 static int records32(b200sph_ctx *ctx, const bool wcsph_list_pass, bool *yes, int *eos_arr)
 {
     *yes = false;
@@ -2290,9 +2316,12 @@ int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_
     int ea = -1;
     if ((rc = records32(ctx, use_lists && !ranged && wcsph_only, &r32, &ea))) return rc;
     const EosTab E32 = ctx->eos_pending;   // (packing the state retires the pending calls)
-    if (r32 != ctx->rec32 || (r32 && E32.rho0[ea] != ctx->rec32_rho0)) {
+    // records packed with another EOS (rho0, c0 or offset; by k_pack_rec32 or, speculatively,
+    // by k_stage_pack) are stale even when the same EOS calls are pending
+    const Rec32Eos key = r32 ? rec32_eos(E32, ea) : Rec32Eos{};
+    if (r32 != ctx->rec32 || (r32 && key != ctx->rec32_eos)) {
         ctx->rec32 = r32;
-        ctx->rec32_rho0 = r32 ? E32.rho0[ea] : 0.0;
+        ctx->rec32_eos = key;
         state_changed(ctx);
     }
     if (!r32 && (rc = ab_positions(ctx))) return rc;
@@ -2362,9 +2391,6 @@ int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_
         pa.rho0 = (float)rho0;
         pa.hrho0 = (float)(0.5 * rho0);
         pa.ac0 = (float)(-0.5 * prog->alpha * c0);
-        pa.kp = (float)(eos_offset(E32, ea) / (rho0 * rho0));
-        const double kB = c0 * c0 / (7.0 * rho0);   // B / rho0^2, B = rho0 c0^2 / gamma
-        pc.tait[0] = (float)kB; pc.tait[1] = (float)(7.0 * kB); pc.tait[2] = (float)(21.0 * kB); pc.tait[3] = (float)(35.0 * kB);
         const double h = pa.h, h1 = 1.0 / h, fac = kernel_fac(ctx->kernel, ctx->dim) * pow(h1, ctx->dim);
         pc.h1 = (float)h1;
         pc.gfac = (float)(fac * h1);
@@ -2719,7 +2745,7 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
         q.rank = ctx->rank; q.key_of = ctx->key_of;
         q.A0 = ctx->A0; q.AB = ctx->AB; q.C = ctx->C;
         q.R = ctx->rec32 ? ctx->R : nullptr;   // the layout the last pair pass read
-        q.rho0 = ctx->rec32_rho0;
+        q.E32 = ctx->rec32_eos;
         q.G = ctx->G;
         q.red_u32 = ctx->red_u32;
         q.dt_cfl = f32_ptr(ctx, B200SPH_DT_CFL); q.dt_force = f32_ptr(ctx, B200SPH_DT_FORCE);

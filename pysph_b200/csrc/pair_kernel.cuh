@@ -26,18 +26,17 @@ struct PairArgs {
     // array (equation.py:448-520); read by the RANGED instantiations of k_pair_list only
     long long doff[B200SPH_MAX_ARRAYS], dlo[B200SPH_MAX_ARRAYS], dhi[B200SPH_MAX_ARRAYS];
     // k_pair_list_r32 only: the 32-byte records, the uniform h and m, and the one Tait EOS
-    // (gamma = 7) of every array: rho = rho0 (1 + delta), cs = c0_eos (1 + delta)^3,
-    // p / rho^2 = (kB ((1 + delta)^7 - 1) + kp) / (1 + delta)^2 with kB = B / rho0^2, kp = p0 / rho0^2;
-    // hrho0 = rho0 / 2, ac0 = -alpha c0_eos / 2.  The kernel's other constants are in PairR32.
+    // (gamma = 7) of every array: rho = rho0 (1 + delta), cs = c0_eos (1 + delta)^3 (p / rho^2
+    // is in the record); hrho0 = rho0 / 2, ac0 = -alpha c0_eos / 2.  The kernel's other
+    // constants are in PairR32.
     const float4 *R;
-    float h, m, rho0, hrho0, ac0, kp;
+    float h, m, rho0, hrho0, ac0;
 };
 
 // The products of uniform values that k_pair_list_r32's loop needs, folded on the host so that
 // the loop reads them as constant-bank operands (a parameter of that kernel alone: the size of
 // PairArgs sets the parameter offsets of every other pair kernel).
 struct PairR32 {
-    float tait[4];     // kB (1, 7, 21, 35): the binomial coefficients of tait_p7
     float h1, gfac, wfac, eta2;   // 1 / h, kfac / h^(DIM + 1) (gradient), kfac / h^DIM (value), 0.01 h^2
     // PairArgs.emask regrouped by equation: per destination type, bit ESEL_X + t says that the
     // Group has equation X (ESEL_ANY: some equation) for source type t

@@ -350,19 +350,11 @@ __global__ void __launch_bounds__(LIST_NT, MINB) k_pair_list(const PairArgs a, c
     }
 }
 
-// kB ((1 + d)^7 - 1) + kp of the Tait EOS (gamma = 7) in Horner form, kB folded into the
-// coefficients: no cancellation for small d
-__device__ __forceinline__ float tait_p7(const PairR32 &c, const float kp, const float d)
-{
-    const float t = fmaf(fmaf(fmaf(fmaf(fmaf(d, c.tait[0], c.tait[1]), d, c.tait[2]), d, c.tait[3]), d, c.tait[3]), d, c.tait[2]);
-    return fmaf(fmaf(t, d, c.tait[1]), d, kp);
-}
-
 // The list consumer of the 32-byte records (records32 in b200sph.cu: the WCSPH scheme's Group
 // with uniform h and m, one Tait EOS with gamma = 7 for every array, no ghosts).  Per entry ONE
-// ld_256 -- a single sector, two 128-bit loads where k_pair_list issues three into two sectors --
-// and what the 48-byte C record carried is recomputed from delta = rho / rho0 - 1: rho, cs and
-// p / rho^2 (one rcp).  h is uniform, so h_ij, 1 / h_ij and the kernel's normalisation are
+// ld_256 -- a single sector, two 128-bit loads where k_pair_list issues three into two sectors.
+// The record carries p / rho^2 (rec32_make) and delta' (delta = rho / rho0 - 1 with the type in
+// its 3 low bits); rho and cs are recomputed from delta' as it is, the type is its low bits.  h is uniform, so h_ij, 1 / h_ij and the kernel's normalisation are
 // uniform constants (PairR32, folded on the host), and the accept test is k_pair_list's on
 // the same floats (the same pairs); m is factored out of the sums.
 // With the records in L2 the loop is bound by the instructions it issues per entry, so the body
@@ -383,9 +375,8 @@ __global__ void __launch_bounds__(LIST_NT, 8) k_pair_list_r32(const PairArgs a, 
     int count = 0;
     if (active) {
         ld_256(a.R + 2 * (size_t)s, Pi, Vi);
-        const int ti = __float_as_int(Vi.w);
-        sel = c.esel[ti & 7];
-        if ((a.real_only && (ti & PT_GHOST)) || !sel) active = false;
+        sel = c.esel[__float_as_int(Vi.w) & 7];
+        if (!sel) active = false;
     }
     if (active) count = (int)cnt[s];
     int cmax = count;
@@ -393,10 +384,10 @@ __global__ void __launch_bounds__(LIST_NT, 8) k_pair_list_r32(const PairArgs a, 
     for (int o = 16; o > 0; o >>= 1) cmax = max(cmax, __shfl_xor_sync(FULL, cmax, o));
     const uint32_t *nxt = lst + ((size_t)(s >> 5) * (size_t)capg) * 32u + (uint32_t)(s & 31);
     const float h2k = a.k2 * a.h * a.h;          // k_pair_list's hi2 (and hj2) on the same floats
-    const float xi = 1.0f + Pi.w, ixi = frcp(xi);
-    const float tmpi = tait_p7(c, a.kp, Pi.w) * (ixi * ixi);                  // p_i / rho_i^2
+    const float xi = 1.0f + Vi.w;
+    const float tmpi = Pi.w;                                             // p_i / rho_i^2
     const float aci = a.ac0 * (xi * xi * xi);                            // -alpha cs_i / 2
-    const float rhoi = fmaf(a.hrho0, Pi.w, a.rho0);                      // rho_ij = rhoi + rho0 delta_j / 2
+    const float rhoi = fmaf(a.hrho0, Vi.w, a.rho0);                      // rho_ij = rhoi + rho0 delta_j / 2
     // cfl: max |h v_ij . x_ij / r^2| over the momentum pairs, -1 while there is none; c0 is added
     // after the loop (rounding is monotonic, so max(t) + c0 == max(t + c0))
     Acc acc = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, -1.f, 0.f};
@@ -409,7 +400,7 @@ __global__ void __launch_bounds__(LIST_NT, 8) k_pair_list_r32(const PairArgs a, 
             const float r2 = entry_dist(a, e, Pi, r.P, xij, yij, zij);
             // the exact accept test, linked_list_nnps.pyx:188, then the Group's equations for the
             // source's type (none: the pair is not counted); without ghosts the type is the array
-            const unsigned eq = (live && r2 < h2k) ? sel >> __float_as_uint(r.V.w) : 0u;
+            const unsigned eq = (live && r2 < h2k) ? sel >> (__float_as_int(r.V.w) & 7) : 0u;
             const bool c_on = eq & (1u << ESEL_CONTINUITY), m_on = eq & (1u << ESEL_MOMENTUM), x_on = eq & (1u << ESEL_XSPH);
             npairs += (eq >> ESEL_ANY) & 1u;
             // pair_body with h_j = h_i = h and m_j = m.  The RIJ > 1e-12 guard of kernels.py:128-132
@@ -422,18 +413,17 @@ __global__ void __launch_bounds__(LIST_NT, 8) k_pair_list_r32(const PairArgs a, 
             const float uij = Vi.x - r.V.x, vij = Vi.y - r.V.y, wwij = Vi.z - r.V.z;
             const float vdotx = uij * xij + vij * yij + wwij * zij;
             acc.arho = fmaf(c_on ? gt : 0.0f, vdotx, acc.arho);
-            const float dj = r.P.w;
+            const float dj = r.V.w;
             const float rhoij1 = frcp(fmaf(a.hrho0, dj, rhoi));
             // momentum, wc/basic.py:215-257
-            const float xj = 1.0f + dj, xj2 = xj * xj;
+            const float xj = 1.0f + dj;
             const float hv = a.h * vdotx;
             const float muij = hv * frcp(r2 + c.eta2);
             // -alpha c_ij mu_ij + beta mu_ij^2, c_ij = (cs_i + cs_j) / 2
-            const float av = muij * fmaf(a.beta, muij, fmaf(a.ac0, xj2 * xj, aci));
+            const float av = muij * fmaf(a.beta, muij, fmaf(a.ac0, xj * xj * xj, aci));
             const float piij = vdotx < 0.0f ? av * rhoij1 : 0.0f;
             acc.cfl = fmaxf(acc.cfl, (m_on && r2 > 1e-12f) ? fabsf(hv * rinv * rinv) : -1.0f);   // + c0 below
-            const float tmpj = tait_p7(c, a.kp, dj) * frcp(xj2);
-            const float f = m_on ? (tmpi + tmpj + piij) * gt : 0.0f;     // times -m below
+            const float f = m_on ? (tmpi + r.P.w + piij) * gt : 0.0f;   // tau_i + tau_j + pi_ij, times -m below
             acc.au = fmaf(f, xij, acc.au);
             acc.av = fmaf(f, yij, acc.av);
             acc.aw = fmaf(f, zij, acc.aw);

@@ -202,8 +202,8 @@ struct FusePackArgs {
     const uint32_t *rank, *key_of;   // pool index -> sorted slot / cell key of the current build
     const float4 *A0;                // packed positions at build time (sorted order)
     float4 *AB, *C;
-    float4 *R;                       // non-null: the state goes into the 32-byte records (rho0: of delta)
-    double rho0;
+    float4 *R;                       // non-null: the state goes into the 32-byte records ...
+    Rec32Eos E32;                    // ... formed with this EOS
     GridDev G;
     unsigned *red_u32;
     const float *dt_cfl, *dt_force;
@@ -213,7 +213,9 @@ struct FusePackArgs {
     EosTab E;
 };
 
-__global__ void __launch_bounds__(256, 5) k_stage_pack(const StageArgs a, const FusePackArgs q)
+// 4 CTAs/SM and no spills: at 5 the kernel spilled (36 B) and ran 7 % slower on H100, and with the
+// 32-byte records carrying p / rho^2 the spill reloads made it 8 % slower again
+__global__ void __launch_bounds__(256, 4) k_stage_pack(const StageArgs a, const FusePackArgs q)
 {
     const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     float d2 = 0.f, dh = 0.f;
@@ -270,7 +272,7 @@ __global__ void __launch_bounds__(256, 5) k_stage_pack(const StageArgs a, const 
                 // only the full sector: a lone 16-byte half would cost a read-modify-write in
                 // HBM per particle (the position half of AB is restored from R on demand, ab_positions)
                 float4 R0, R1;
-                rec32_make(A, un, vn, wn, r, q.eos_any && q.E.on[ar] && q.E.hg[ar], q.rho0, (int)t, R0, R1);
+                rec32_make(A, un, vn, wn, r, q.eos_any && q.E.on[ar] && q.E.hg[ar], q.E32, (int)t, R0, R1);
                 q.R[2 * (size_t)s] = R0;
                 q.R[2 * (size_t)s + 1] = R1;
             } else {
@@ -376,7 +378,7 @@ __global__ void k_pack_rec32(const double *__restrict__ u, const double *__restr
                              const double *__restrict__ w, double *__restrict__ rho, float *__restrict__ p,
                              float *__restrict__ cs, const uint8_t *__restrict__ ptype,
                              const uint32_t *__restrict__ perm, long long n, const float4 *__restrict__ AB,
-                             float4 *__restrict__ R, const EosTab E, const double rho0)
+                             float4 *__restrict__ R, const EosTab E, const Rec32Eos E32)
 {
     long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n) return;
@@ -384,7 +386,7 @@ __global__ void k_pack_rec32(const double *__restrict__ u, const double *__restr
     const uint8_t t = ptype[g];
     eos_tab_apply(rho, p, cs, t, g, E);
     float4 R0, R1;
-    rec32_make(AB[2 * s], u[g], v[g], w[g], rho[g], E.on[t & 7] && E.hg[t & 7], rho0, (int)t, R0, R1);
+    rec32_make(AB[2 * s], u[g], v[g], w[g], rho[g], E.on[t & 7] && E.hg[t & 7], E32, (int)t, R0, R1);
     R[2 * s] = R0;
     R[2 * s + 1] = R1;
 }

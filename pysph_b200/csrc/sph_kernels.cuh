@@ -13,16 +13,17 @@ template <int DIM> __device__ __forceinline__ float hpow(float h1)
 
 template <int K> __device__ __forceinline__ void sph_kernel(float q, float &w, float &dw);
 
-// CubicSpline kernels.py:69-124
+// CubicSpline kernels.py:69-124, as clamped truncated powers (no compares, no selects): with
+// t = clamp(1 - q/2, 0, 1) and s = clamp(1 - q, 0, 1), w = 2 t^3 - s^3 and dw = -3 min(q/2, t) (s + t)
+// for every q >= 0 (q > 2 included).  The product form of dw equals 3 (s^2 - t^2) without its
+// cancellation near q = 0.  The clamps compile to .SAT.
 template <> __device__ __forceinline__ void sph_kernel<0>(float q, float &w, float &dw)
 {
-    const float t2 = 2.0f - q;
-    const float w_in = 1.0f - 1.5f * q * q * (1.0f - 0.5f * q);
-    const float d_in = -3.0f * q * (1.0f - 0.75f * q);
-    const float w_out = 0.25f * t2 * t2 * t2;
-    const float d_out = -0.75f * t2 * t2;
-    w = q > 2.0f ? 0.0f : (q > 1.0f ? w_out : w_in);
-    dw = q > 2.0f ? 0.0f : (q > 1.0f ? d_out : d_in);
+    const float hq = 0.5f * q;
+    const float t = fminf(fmaxf(1.0f - hq, 0.0f), 1.0f);
+    const float s = fminf(fmaxf(1.0f - q, 0.0f), 1.0f);
+    w = 2.0f * (t * t * t) - s * s * s;
+    dw = -3.0f * fminf(hq, t) * (s + t);
 }
 // WendlandQuintic kernels.py:304-343
 template <> __device__ __forceinline__ void sph_kernel<1>(float q, float &w, float &dw)
