@@ -389,6 +389,16 @@ int b200sph_time_get(b200sph_ctx *ctx, double out[2]);
  * sweep over the state.  Results are bitwise those of the separate kernels; the pool's
  * rho / p / cs change only when the next evaluation issues its b200sph_eos calls. */
 int b200sph_stage_dev(b200sph_ctx *ctx, int arr, int which);
+/* WCSPHTVDRK3Step integrator_step.py:96-168 (TVDRK3Integrator, integrator.py:426-460); which:
+ * 0 initialize (WCSPHStep's), 1 stage1 q = q0 + dt aq, 2 stage2 q = 3/4 q0 + 1/4 (q + dt aq),
+ * 3 stage3 q = 1/3 q0 + 2/3 (q + dt aq); every stage uses the whole dt.  The fast path is that
+ * of b200sph_stage_dev (k_stage_pack_rk3, same conditions and results bitwise those of the
+ * separate kernels), with the adaptive-dt factors reduced after stage3, the end of the step.
+ * These two entries are new symbols only: no structure and no b200sph_stats counter changed,
+ * so B200SPH_ABI_VERSION stays 5. */
+int b200sph_stage_rk3(b200sph_ctx *ctx, int arr, int which, double dt);
+/* the same with dt read from the device-resident time-control block */
+int b200sph_stage_rk3_dev(b200sph_ctx *ctx, int arr, int which);
 /* enqueue: reduce dt_cfl / dt_force / h, then block[2] = cfl * min(hmin / max_cfl,
  * sqrt(hmin / sqrt(max_force))), or 1e20 when nothing constrains it (solver.py:655-660);
  * fixed_h keeps the first hmin (integrator.py:170-176) */

@@ -8,7 +8,8 @@ mirror the reference's plugin seam for this path:
 reference (pypr/pysph)      here
 ==========================  ==================================================
 compiled AccelerationEval   :class:`B200AccelerationEval`
-compiled Integrator         :class:`PECIntegrator`, :class:`EPECIntegrator`
+compiled Integrator         :class:`PECIntegrator`, :class:`EPECIntegrator`,
+                            :class:`TVDRK3Integrator`
 NNPS (LinkedListNNPS)       :class:`B200NNPS`
 DeviceHelper (``pa.gpu``)   :class:`B200DeviceHelper` / :class:`B200Backend`
 Equation / Group            :mod:`pysph_b200.equations`
@@ -35,7 +36,7 @@ from .domain import DomainManager
 from .nnps import B200NNPS
 from .acceleration_eval import B200AccelerationEval
 from .integrator import (B200Integrator, PECIntegrator, EPECIntegrator,
-                         WCSPHStep)
+                         TVDRK3Integrator, WCSPHStep, WCSPHTVDRK3Step)
 from .solver import B200Solver
 from .edac import EDACScheme, EDACTVFStep, EDACStep
 from .output import dump, load
@@ -54,8 +55,12 @@ def make_wcsph_solver(particles, params, kernel, device=0, **solver_kw):
     cfl = p.pop('cfl', 0.3)
     scheme = WCSPHScheme(**p)
     names = scheme.fluids + scheme.solids
-    cls = {'EPEC': EPECIntegrator, 'PEC': PECIntegrator}[integ_name]
-    integrator = cls(**dict((n, WCSPHStep()) for n in names))
+    cls = {'EPEC': EPECIntegrator, 'PEC': PECIntegrator,
+           'TVDRK3': TVDRK3Integrator}[integ_name]
+    # WCSPHScheme.configure_solver (scheme.py:360-386): TVD-RK3 steps every array with
+    # WCSPHTVDRK3Step
+    step_cls = WCSPHTVDRK3Step if cls is TVDRK3Integrator else WCSPHStep
+    integrator = cls(**dict((n, step_cls()) for n in names))
     kw = dict(adaptive_timestep=True, cfl=cfl, n_damp=n_damp, tf=1e9,
               fixed_h=not p.get('update_h', False), device=device)
     kw.update(solver_kw)

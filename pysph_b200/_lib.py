@@ -168,6 +168,8 @@ SIGNATURES = {
     'b200sph_time_set': (C.c_int, [_ctx_p, C.c_double, C.c_double]),
     'b200sph_time_get': (C.c_int, [_ctx_p, _dp]),
     'b200sph_stage_dev': (C.c_int, [_ctx_p, C.c_int, C.c_int]),
+    'b200sph_stage_rk3': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_double]),
+    'b200sph_stage_rk3_dev': (C.c_int, [_ctx_p, C.c_int, C.c_int]),
     'b200sph_dt_propose': (C.c_int, [_ctx_p, C.c_double, C.c_int]),
     'b200sph_dt_commit': (C.c_int, [_ctx_p, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int]),
     'b200sph_dt_advance': (C.c_int, [_ctx_p, C.c_double, C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int]),

@@ -2643,16 +2643,18 @@ int b200sph_solid_pass(b200sph_ctx *ctx, const b200sph_solid_program *prog, int6
 }
 
 static int ensure_tc(b200sph_ctx *ctx);
-// what every stage entry point (WCSPHStep, the EDAC steppers, SolidMechStep) checks and
-// prepares before it fills its arguments
-static int stage_begin(b200sph_ctx *ctx, const char *who, int arr, int which, bool devdt)
+// what every stage entry point (WCSPHStep, WCSPHTVDRK3Step, the EDAC steppers, SolidMechStep)
+// checks and prepares before it fills its arguments; `last` is the stepper's last stage
+static int stage_begin(b200sph_ctx *ctx, const char *who, int arr, int which, bool devdt, int last = 2)
 {
     if (int rcc = require_confirmed(ctx, who)) return rcc;
     CU(cudaSetDevice(ctx->device));
     int rc = ensure_pool(ctx);
     if (rc) return rc;
     if (arr >= ctx->narr) return set_err(ctx, "%s: bad array %d", who, arr);
-    if (which < 0 || which > 2) return set_err(ctx, "%s: which must be 0 (initialize), 1 (stage1) or 2 (stage2)", who);
+    if (last == 3 && (which < 0 || which > 3))
+        return set_err(ctx, "%s: which must be 0 (initialize), 1 (stage1), 2 (stage2) or 3 (stage3)", who);
+    if (which < 0 || which > last) return set_err(ctx, "%s: which must be 0 (initialize), 1 (stage1) or 2 (stage2)", who);
     if (devdt && (rc = ensure_tc(ctx))) return rc;
     return 0;
 }
@@ -2728,16 +2730,20 @@ static bool can_fuse_stage(const b200sph_ctx *ctx, int arr)
     return ntot == ctx->n_sorted && lists_usable(ctx, ntot);
 }
 
-static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devdt)
+// WCSPHStep (rk3 = false: stages 1, 2) and WCSPHTVDRK3Step (rk3: stages 1, 2, 3); the dt
+// factors belong to the evaluation before the stepper's last stage
+static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devdt, bool rk3 = false)
 {
-    int rc = stage_begin(ctx, "stage", arr, which, devdt);
+    const int last = rk3 ? 3 : 2;
+    int rc = stage_begin(ctx, rk3 ? "stage_rk3" : "stage", arr, which, devdt, last);
     if (rc || (rc = eos_flush(ctx))) return rc;
     PhaseTimer pt(ctx, 2);
     StageArgs sa;
     stage_args(ctx, sa, arr, which, dt);
+    if (rk3) sa.f = dt;   // every TVD-RK3 stage takes the whole dt
     sa.rho = ctx->f64[B200SPH_RHO]; sa.rho0 = ctx->f64[B200SPH_RHO0]; sa.arho = f32_ptr(ctx, B200SPH_ARHO);
     if (which != 0 && ctx->pool_end > 0 && can_fuse_stage(ctx, arr)) {
-        // stage + records of the next evaluation (+ the dt factors after stage2) in one pass
+        // stage + records of the next evaluation (+ the dt factors after the last stage) in one pass
         FusePackArgs q;
         memset(&q, 0, sizeof(q));
         q.h = ctx->f64[B200SPH_H]; q.m = ctx->f64[B200SPH_M];
@@ -2752,7 +2758,7 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
         q.red = ctx->red;
         q.tc = devdt ? ctx->tc : nullptr;
         q.do_init = 0;
-        q.reduce_dt = (which == 2 && ctx->dt_adaptive_seen) ? 1 : 0;
+        q.reduce_dt = (which == last && ctx->dt_adaptive_seen) ? 1 : 0;
         q.eos_any = ctx->eos_last_valid ? 1 : 0;
         q.E = ctx->eos_last;
         if (q.reduce_dt && !ctx->red_armed) {
@@ -2760,11 +2766,12 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
             LAUNCH_CHECK();
         }
         CU(cudaMemsetAsync(ctx->red_u32, 0, 2 * sizeof(unsigned), ctx->stream));
-        k_stage_pack<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa, q);
+        if (rk3) k_stage_pack_rk3<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa, q);
+        else k_stage_pack<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa, q);
         LAUNCH_CHECK();
         ctx->n_fused++;
         if (q.reduce_dt) ctx->red_armed = false;
-        if (which == 2) ctx->dt_reduced = q.reduce_dt != 0, ctx->dt_adaptive_seen = false;
+        if (which == last) ctx->dt_reduced = q.reduce_dt != 0, ctx->dt_adaptive_seen = false;
         positions_changed(ctx);        // particles moved: nnps_update must decide about the lists
         ctx->packed_valid = true;      // ... but their packed positions are current,
         ctx->ab_stale = q.R != nullptr;    // (in R only, with the 32-byte records)
@@ -2775,17 +2782,23 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
         return 0;
     }
     if (ctx->pool_end > 0) {
-        if (devdt) k_stage_devdt<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa, ctx->tc);
-        else k_stage<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
+        const unsigned nb = (unsigned)cdiv(ctx->pool_end, 256);
+        if (rk3 && which != 0) {
+            if (devdt) k_stage_rk3_devdt<<<nb, 256, 0, ctx->stream>>>(sa, ctx->tc);
+            else k_stage_rk3<<<nb, 256, 0, ctx->stream>>>(sa);
+        } else if (devdt) k_stage_devdt<<<nb, 256, 0, ctx->stream>>>(sa, ctx->tc);
+        else k_stage<<<nb, 256, 0, ctx->stream>>>(sa);
         LAUNCH_CHECK();
     }
     if (which != 0) particles_moved(ctx);
-    if (which == 2) ctx->dt_adaptive_seen = false, ctx->dt_reduced = false;
+    if (which == last) ctx->dt_adaptive_seen = false, ctx->dt_reduced = false;
     return 0;
 }
 
 int b200sph_stage(b200sph_ctx *ctx, int arr, int which, double dt) { return stage_impl(ctx, arr, which, dt, false); }
 int b200sph_stage_dev(b200sph_ctx *ctx, int arr, int which) { return stage_impl(ctx, arr, which, 0.0, true); }
+int b200sph_stage_rk3(b200sph_ctx *ctx, int arr, int which, double dt) { return stage_impl(ctx, arr, which, dt, false, true); }
+int b200sph_stage_rk3_dev(b200sph_ctx *ctx, int arr, int which) { return stage_impl(ctx, arr, which, 0.0, true, true); }
 
 // ---- device-resident time step ------------------------------------------------
 int b200sph_time_control(b200sph_ctx *ctx, double *external_block8, double **dev_block)

@@ -180,18 +180,20 @@ __device__ __forceinline__ void stage_body(const StageArgs &a)
 }
 
 // ---------------------------------------------------------------------------
-// The fused stage kernel of the WCSPH fast path (every array steps with WCSPHStep, the
-// neighbour lists of the current build are reusable): in ONE pass over the pool, per real
-// particle,
+// The fused stage kernels of the WCSPH fast path (every array steps with WCSPHStep:
+// k_stage_pack, or with WCSPHTVDRK3Step: k_stage_pack_rk3; the neighbour lists of the current
+// build are reusable): in ONE pass over the pool, per real particle,
 //   [initialize (integrator_step.py:51-61) when it was deferred to here]
 //   stage1 / stage2 (integrator_step.py:63-91), fp64, bitwise what k_stage computes
+//     (k_stage_pack_rk3: stage1 / stage2 / stage3, :118-168, bitwise what k_stage_rk3 computes)
 //   the packed pair records of the NEXT evaluation at the particle's sorted slot:
 //     {A, B} = (cell-relative position of the frozen build, h, u, v, w, m)   -- k_pack_pos_light
 //     C      = (rho, p / rho^2, cs, type) with the equation-of-state calls of the LAST
 //              evaluation applied to the record only (k_pack_state's arithmetic); the pool's
 //              rho / p / cs are written when the evaluation really issues those calls
 //   the drift of the build (max |x - x_build|^2, max (h - h_build)) into red_u32
-//   [stage2: the adaptive-dt factors max dt_cfl, max dt_force, min h into red[9,11,12]]
+//   [the stepper's last stage: the adaptive-dt factors max dt_cfl, max dt_force, min h into
+//    red[9,11,12]]
 // It replaces k_stage + k_stage(initialize) + k_pack_pos_light + k_pack_state (+ k_reduce_dt):
 // five sweeps over the fp64 state become one.  Ghost particles are not stepped
 // (integrator_cython.mako:97-111) and their records are refreshed by the halo scatter.
@@ -213,9 +215,47 @@ struct FusePackArgs {
     EosTab E;
 };
 
-// 4 CTAs/SM and no spills: at 5 the kernel spilled (36 B) and ran 7 % slower on H100, and with the
-// 32-byte records carrying p / rho^2 the spill reloads made it 8 % slower again
-__global__ void __launch_bounds__(256, 4) k_stage_pack(const StageArgs a, const FusePackArgs q)
+// WCSPHTVDRK3Step.stage1 / stage2 / stage3 (integrator_step.py:118-168) for one property, in the
+// reference's association order; q is read by stages 2 and 3 only.  k_stage_rk3 and
+// k_stage_pack_rk3 both call it, so that both contract it to the same FMAs.
+__device__ __forceinline__ double rk3_update(const int which, const double q0, const double *q,
+                                             const long long g, const double dt, const float aq)
+{
+    if (which == 1) return q0 + dt * (double)aq;
+    if (which == 2) return 0.75 * q0 + 0.25 * (q[g] + dt * (double)aq);
+    return (1. / 3.) * q0 + (2. / 3.) * (q[g] + dt * (double)aq);
+}
+
+// WCSPHTVDRK3Step stage1 / stage2 / stage3 (a.which = 1, 2, 3) with dt = a.f, real particles only;
+// its initialize is WCSPHStep's (k_stage, which = 0)
+__device__ __forceinline__ void stage_rk3_body(const StageArgs &a)
+{
+    long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= a.pool_end) return;
+    uint8_t t = a.ptype[g];
+    if (t == PT_INVALID || (t & PT_GHOST)) return;
+    if (a.arr >= 0 && (t & 7) != a.arr) return;
+    const double dt = a.f;
+    a.u[g] = rk3_update(a.which, a.u0[g], a.u, g, dt, a.au[g]);
+    a.v[g] = rk3_update(a.which, a.v0[g], a.v, g, dt, a.av[g]);
+    a.w[g] = rk3_update(a.which, a.w0[g], a.w, g, dt, a.aw[g]);
+    a.x[g] = rk3_update(a.which, a.x0[g], a.x, g, dt, a.ax[g]);
+    a.y[g] = rk3_update(a.which, a.y0[g], a.y, g, dt, a.ay[g]);
+    a.z[g] = rk3_update(a.which, a.z0[g], a.z, g, dt, a.az[g]);
+    a.rho[g] = rk3_update(a.which, a.rho0[g], a.rho, g, dt, a.arho[g]);
+}
+__global__ void k_stage_rk3(StageArgs a) { stage_rk3_body(a); }
+__global__ void k_stage_rk3_devdt(StageArgs a, const double *__restrict__ tc)
+{
+    a.f = tc[0];
+    stage_rk3_body(a);
+}
+
+// The body of the fused stage kernels, the stage being WCSPHStep's or, RK3, WCSPHTVDRK3Step's.
+// s_* is the kernel's shared memory of the block reduction (one atomic per block and quantity).
+template <bool RK3>
+__device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePackArgs &q, float *s_d2, float *s_dh,
+                                                double *s_mc, double *s_mf, double *s_hm)
 {
     const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     float d2 = 0.f, dh = 0.f;
@@ -228,7 +268,7 @@ __global__ void __launch_bounds__(256, 4) k_stage_pack(const StageArgs a, const 
             double f = a.f;
             if (q.tc) {
                 const double dt = q.tc[0];
-                f = a.which == 1 ? 0.5 * dt : dt;
+                f = RK3 ? dt : (a.which == 1 ? 0.5 * dt : dt);
             }
             double x0, y0, z0, u0, v0, w0, r0;
             if (q.do_init) {
@@ -243,13 +283,24 @@ __global__ void __launch_bounds__(256, 4) k_stage_pack(const StageArgs a, const 
                 u0 = a.u0[g]; v0 = a.v0[g]; w0 = a.w0[g];
                 r0 = a.rho0[g];
             }
-            const double un = u0 + f * (double)a.au[g];
-            const double vn = v0 + f * (double)a.av[g];
-            const double wn = w0 + f * (double)a.aw[g];
-            const double xn = x0 + f * (double)a.ax[g];
-            const double yn = y0 + f * (double)a.ay[g];
-            const double zn = z0 + f * (double)a.az[g];
-            double r = r0 + f * (double)a.arho[g];
+            double un, vn, wn, xn, yn, zn, r;
+            if (RK3) {
+                un = rk3_update(a.which, u0, a.u, g, f, a.au[g]);
+                vn = rk3_update(a.which, v0, a.v, g, f, a.av[g]);
+                wn = rk3_update(a.which, w0, a.w, g, f, a.aw[g]);
+                xn = rk3_update(a.which, x0, a.x, g, f, a.ax[g]);
+                yn = rk3_update(a.which, y0, a.y, g, f, a.ay[g]);
+                zn = rk3_update(a.which, z0, a.z, g, f, a.az[g]);
+                r = rk3_update(a.which, r0, a.rho, g, f, a.arho[g]);
+            } else {
+                un = u0 + f * (double)a.au[g];
+                vn = v0 + f * (double)a.av[g];
+                wn = w0 + f * (double)a.aw[g];
+                xn = x0 + f * (double)a.ax[g];
+                yn = y0 + f * (double)a.ay[g];
+                zn = z0 + f * (double)a.az[g];
+                r = r0 + f * (double)a.arho[g];
+            }
             a.u[g] = un; a.v[g] = vn; a.w[g] = wn;
             a.x[g] = xn; a.y[g] = yn; a.z[g] = zn;
             a.rho[g] = r;
@@ -317,9 +368,6 @@ __global__ void __launch_bounds__(256, 4) k_stage_pack(const StageArgs a, const 
             hm = fmin(hm, __shfl_xor_sync(0xffffffffu, hm, o));
         }
     }
-    // one atomic per block and quantity
-    __shared__ float s_d2[8], s_dh[8];
-    __shared__ double s_mc[8], s_mf[8], s_hm[8];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (lane == 0) {
         s_d2[warp] = d2; s_dh[warp] = dh;
@@ -339,6 +387,24 @@ __global__ void __launch_bounds__(256, 4) k_stage_pack(const StageArgs a, const 
             if (hm < 1e299) atomicMin(&q.red[12], d2o(hm));
         }
     }
+}
+
+// 4 CTAs/SM and no spills: at 5 the kernel spilled (36 B) and ran 7 % slower on H100, and with the
+// 32-byte records carrying p / rho^2 the spill reloads made it 8 % slower again
+__global__ void __launch_bounds__(256, 4) k_stage_pack(const StageArgs a, const FusePackArgs q)
+{
+    __shared__ float s_d2[8], s_dh[8];
+    __shared__ double s_mc[8], s_mf[8], s_hm[8];
+    stage_pack_body<false>(a, q, s_d2, s_dh, s_mc, s_mf, s_hm);
+}
+
+// k_stage_pack for WCSPHTVDRK3Step (which = 1, 2, 3; dt is used whole): stages 2 and 3 read
+// the current state as well as the stage copies.  61 registers, no spills at 4 CTAs/SM.
+__global__ void __launch_bounds__(256, 4) k_stage_pack_rk3(const StageArgs a, const FusePackArgs q)
+{
+    __shared__ float s_d2[8], s_dh[8];
+    __shared__ double s_mc[8], s_mf[8], s_hm[8];
+    stage_pack_body<true>(a, q, s_d2, s_dh, s_mc, s_mf, s_hm);
 }
 
 // TaitEOS.loop wc/basic.py:60-65 ; TaitEOSHGCorrection.loop wc/basic.py:118-126: the pending

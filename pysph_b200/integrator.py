@@ -8,8 +8,8 @@ arguments, then ``set_acceleration_evals`` / ``set_nnps`` /
 from integrator_cython.mako:87-112 are the ``k_stage`` CUDA kernel; the stage
 ordering of ``one_timestep`` follows integrator.py:322-420.
 
-Only ``WCSPHStep`` (integrator_step.py:38-91) has a device kernel; another
-stepper class raises at construction.
+Each integrator accepts the steppers it has device kernels for (``steppers``);
+another stepper class raises at construction.
 """
 from math import sqrt
 
@@ -25,23 +25,33 @@ class WCSPHStep(IntegratorStep):
     pysph/sph/integrator_step.py:38-91 (device kernel: k_stage)."""
 
 
+class WCSPHTVDRK3Step(IntegratorStep):
+    """TVD-RK3 stepper: initialize / stage1 / stage2 / stage3 of
+    pysph/sph/integrator_step.py:96-168 (device kernel: k_stage_rk3)."""
+
+
 # stepper class name -> (C-ABI stage call, the same with dt read on the device)
 _SUPPORTED_STEPPERS = {
     'WCSPHStep': ('b200sph_stage', 'b200sph_stage_dev'),
     'EDACTVFStep': ('b200sph_stage_tvf', 'b200sph_stage_tvf_dev'),   # wc/edac.py:491-540
     'EDACStep': ('b200sph_stage_edac', 'b200sph_stage_edac_dev'),    # wc/edac.py:82-133
     'SolidMechStep': ('b200sph_stage_solid', 'b200sph_stage_solid_dev'),   # integrator_step.py:173-252
+    'WCSPHTVDRK3Step': ('b200sph_stage_rk3', 'b200sph_stage_rk3_dev'),
 }
 
 
 class B200Integrator(object):
+    # the predictor-corrector steppers (two stages)
+    steppers_supported = ('WCSPHStep', 'EDACTVFStep', 'EDACStep', 'SolidMechStep')
+
     def __init__(self, **kw):
         for name, stepper in kw.items():
             cls = stepper.__class__.__name__
-            if cls not in _SUPPORTED_STEPPERS:
+            if cls not in self.steppers_supported:
                 raise NotImplementedError(
-                    'B200 backend: no device kernel for stepper %r of array '
-                    '%r (supported: %s)' % (cls, name, tuple(_SUPPORTED_STEPPERS)))
+                    'B200 backend: no device kernel for stepper %r of array %r under '
+                    '%s (supported: %s)' % (cls, name, self.__class__.__name__,
+                                            self.steppers_supported))
         self.steppers = kw
         self.acceleration_evals = None
         self.nnps = None
@@ -105,6 +115,9 @@ class B200Integrator(object):
 
     def stage2(self):
         self._stage(2, self.dt)
+
+    def stage3(self):
+        self._stage(3, self.dt)
 
     def do_post_stage(self, stage_dt, stage):
         # integrator_cython.mako:59-74
@@ -204,3 +217,37 @@ class EPECIntegrator(B200Integrator):
         self.stage2()
         self.update_domain()
         self.do_post_stage(dt, 2)
+
+
+class TVDRK3Integrator(B200Integrator):
+    """TVD-RK3 (integrator.py:426-460) with WCSPHTVDRK3Step: three evaluations
+    per step; every stage advances by the whole dt from a combination of the
+    stage copies and the current state, and the post-stage times are dt/3,
+    2dt/3 and dt as in the reference."""
+    steppers_supported = ('WCSPHTVDRK3Step',)
+
+    def set_nnps(self, nnps):
+        if getattr(getattr(nnps, 'domain', None), 'is_periodic', False):
+            # update_domain box-wraps x, y, z but not x0, y0, z0 (nnps_base.pyx:699-743):
+            # stages 2 and 3 would combine q0 with a wrapped q and displace a particle
+            # that crossed a periodic face by a fraction of the box
+            raise NotImplementedError(
+                'B200 backend: TVDRK3Integrator in a periodic domain (the periodic wrap '
+                'moves x, y, z but not the stage copies x0, y0, z0 that stages 2 and 3 '
+                'combine them with)')
+        B200Integrator.set_nnps(self, nnps)
+
+    def one_timestep(self, t, dt):
+        self.initialize()
+        self.compute_accelerations()
+        self.stage1()
+        self.update_domain()
+        self.do_post_stage(1. / 3 * dt, 1)
+        self.compute_accelerations()
+        self.stage2()
+        self.update_domain()
+        self.do_post_stage(2. / 3 * dt, 2)
+        self.compute_accelerations()
+        self.stage3()
+        self.update_domain()
+        self.do_post_stage(dt, 3)
