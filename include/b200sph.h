@@ -387,7 +387,11 @@ int b200sph_time_get(b200sph_ctx *ctx, double out[2]);
  * the last evaluation applied to the records) and, after stage2, reduces the adaptive-dt
  * factors -- the work of k_stage + k_pack_pos_light + k_pack_state + k_reduce_dt in one
  * sweep over the state.  Results are bitwise those of the separate kernels; the pool's
- * rho / p / cs change only when the next evaluation issues its b200sph_eos calls. */
+ * rho / p / cs change only when the next evaluation issues its b200sph_eos calls.  On the same
+ * path which = 0 (initialize) launches nothing: the next fused stage copies x .. rho into
+ * x0 .. rho0 as it goes, and applies the pool side of the last evaluation's EOS calls (the
+ * pair pass leaves it to that kernel).  Every other entry point that could observe either runs
+ * it first, so what the host can pull is the same as with the separate kernels. */
 int b200sph_stage_dev(b200sph_ctx *ctx, int arr, int which);
 /* WCSPHTVDRK3Step integrator_step.py:96-168 (TVDRK3Integrator, integrator.py:426-460); which:
  * 0 initialize (WCSPHStep's), 1 stage1 q = q0 + dt aq, 2 stage2 q = 3/4 q0 + 1/4 (q + dt aq),

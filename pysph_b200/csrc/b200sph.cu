@@ -297,6 +297,10 @@ struct b200sph_ctx {
 
     EosTab eos_pending;
     bool eos_any = false;
+    // the pool side (rho clamp, p, cs) of EOS calls a pair pass has already put into the records,
+    // left for the next fused stage kernel; eos_flush runs it stand-alone (before eos_pending)
+    EosTab eos_pool;
+    bool eos_pool_any = false;
     // ---- peer protocol (b200sph_peer_*) + interior / boundary split of the list consumer --
     int peer_rank = -1, peer_world = 0;
     struct PeerBox *peer_box = nullptr;          // this rank's mailbox
@@ -344,6 +348,7 @@ struct b200sph_ctx {
     bool red_armed = false;      // red[9,11,12] hold their neutral values
     bool dt_reduced = false;     // ... hold the factors of the last evaluation (fused stage2)
     bool dt_adaptive_seen = false;  // a dt proposal followed the last stage2: reduce in the next one
+    bool init_pending = false;   // an initialize of every array waits for the next fused stage (init_materialise)
     int64_t n_fused = 0;
 
     // stats
@@ -775,12 +780,17 @@ static int sync_comm(b200sph_ctx *ctx)
     return 0;
 }
 
-static int ensure_pool(b200sph_ctx *ctx, bool join = true)
+static int init_materialise(b200sph_ctx *ctx);
+// every entry point starts here; all but those of the time step's fast path (pair_pass, eos,
+// nnps_update, the WCSPH stages: keep_init) first run a deferred initialize
+static int ensure_pool(b200sph_ctx *ctx, bool join = true, bool keep_init = false)
 {
     if (join) {
         int rc0 = sync_comm(ctx);
         if (rc0) return rc0;
     }
+    if (!keep_init)
+        if (int rci = init_materialise(ctx)) return rci;
     if (ctx->pool_cap == 0) {
         int64_t caps[B200SPH_MAX_ARRAYS];
         for (int a = 0; a < ctx->narr; a++) caps[a] = std::max(ctx->arr[a].cap, ctx->arr[a].n);
@@ -883,6 +893,28 @@ template <class S> static void stage_args(b200sph_ctx *ctx, S &sa, int arr, int 
     sa.arr = arr;
     sa.which = which;
     sa.f = which == 1 ? 0.5 * dt : dt;
+}
+
+// ---- the deferred initialize ----------------------------------------------------------------
+// WCSPHStep.initialize of every array (WCSPHTVDRK3Step's is the same) copies x .. rho into
+// x0 .. rho0.  When the stage that follows will be the fused kernel, stage_impl only records it
+// (init_pending) and that kernel copies as it goes (do_init): one sweep over the state less per
+// step.  The one rule: whatever could observe the copy not being made yet -- reads x0 .. rho0,
+// writes x .. rho, applies EOS calls to the pool's rho (eos_flush, pack_state), changes the
+// particle set or the stream -- runs it here first, as k_stage(0) on the state as it is, which is
+// the state the initialize saw.  ensure_pool does so for every entry point outside the fast path.
+static int init_materialise(b200sph_ctx *ctx)
+{
+    if (!ctx->init_pending) return 0;
+    ctx->init_pending = false;
+    StageArgs sa;
+    stage_args(ctx, sa, -1, 0, 0.0);
+    sa.rho = ctx->f64[B200SPH_RHO]; sa.rho0 = ctx->f64[B200SPH_RHO0]; sa.arho = f32_ptr(ctx, B200SPH_ARHO);
+    if (ctx->pool_end > 0) {
+        k_stage<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
+        LAUNCH_CHECK();
+    }
+    return 0;
 }
 
 // the pair counter of a pass that reports its pair count (pairs_out != null)
@@ -1043,6 +1075,7 @@ const char *b200sph_last_error(b200sph_ctx *ctx)
 int b200sph_set_stream(b200sph_ctx *ctx, void *s)
 {
     CU(cudaSetDevice(ctx->device));
+    if (int rci = init_materialise(ctx)) return rci;
     CU(cudaStreamSynchronize(ctx->stream));
     if (ctx->own_stream) CU(cudaStreamDestroy(ctx->stream));
     if (s) {
@@ -1068,6 +1101,7 @@ int b200sph_add_array(b200sph_ctx *ctx, const char *name, int64_t n, int64_t n_r
     if (ctx->narr >= B200SPH_MAX_ARRAYS) return set_err(ctx, "too many particle arrays (max %d)", B200SPH_MAX_ARRAYS);
     if (n < 0 || n_real < 0 || n_real > n) return set_err(ctx, "add_array: bad sizes n=%lld n_real=%lld", (long long)n, (long long)n_real);
     CU(cudaSetDevice(ctx->device));
+    if (int rci = init_materialise(ctx)) return rci;   // (before the layout moves)
     const int a = ctx->narr;
     ctx->arr[a].name = name ? name : "";
     ctx->arr[a].n = n;
@@ -1093,6 +1127,7 @@ int b200sph_resize_array(b200sph_ctx *ctx, int arr, int64_t n, int64_t n_real)
     if (arr < 0 || arr >= ctx->narr) return set_err(ctx, "resize_array: bad array %d", arr);
     if (n < 0 || n_real < 0 || n_real > n) return set_err(ctx, "resize_array: bad sizes");
     CU(cudaSetDevice(ctx->device));
+    if (int rci = init_materialise(ctx)) return rci;
     { int rc0 = eos_flush(ctx); if (rc0) return rc0; }
     if (ctx->pool_cap == 0) {
         ctx->arr[arr].cap = std::max(ctx->arr[arr].cap, n);
@@ -1615,7 +1650,8 @@ int b200sph_nnps_update(b200sph_ctx *ctx)
     // with the peer protocol's refresh in flight the only thing this call may do without
     // waiting for it is to accept the build the ranks have (speculatively) agreed to keep
     int rc = ensure_pool(ctx, !(ctx->comm_pending && ctx->drift_ok && ctx->packed_valid && reusable_build(ctx) &&
-                                !ctx->eos_any && ctx->domain_valid && !ctx->check_pending));
+                                !ctx->eos_any && ctx->domain_valid && !ctx->check_pending),
+                     true);
     if (rc) return rc;
     if (ctx->check_pending) {   // update after update without an evaluation in between
         int redo = 0;
@@ -1937,18 +1973,35 @@ int b200sph_get_grid(b200sph_ctx *ctx, b200sph_grid_info *out)
     return 0;
 }
 
+// the pool side of the EOS calls a pair pass left for the fused stage kernel, stand-alone
+static int eos_pool_flush(b200sph_ctx *ctx, cudaStream_t s)
+{
+    if (!ctx->eos_pool_any) return 0;
+    if (ctx->pool_end > 0) {
+        k_eos_tab<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, s>>>(ctx->f64[B200SPH_RHO], f32_ptr(ctx, B200SPH_P),
+                                                                      f32_ptr(ctx, B200SPH_CS), ctx->ptype, ctx->pool_end, ctx->eos_pool);
+        LAUNCH_CHECK();
+    }
+    ctx->eos_pool_any = false;
+    return 0;
+}
+
 // run the pending equation-of-state calls stand-alone (something needs rho/p/cs now, or the
 // packed records already hold them: the pool side of a speculated EOS) -- one launch
 static int eos_flush(b200sph_ctx *ctx, cudaStream_t on_comm_stream)
 {
-    if (!ctx->eos_any) return 0;
+    if (!ctx->eos_any && !ctx->eos_pool_any) return 0;
     // ghost rho may be in the middle of a refresh: wait for it -- unless the caller puts
     // this launch on the communication stream itself, behind the scatter
     if (!on_comm_stream)
         if (int rcj = sync_comm(ctx)) return rcj;
+    if (int rci = init_materialise(ctx)) return rci;   // (it copies the rho of before these calls)
+    cudaStream_t s = on_comm_stream ? on_comm_stream : ctx->stream;
+    if (int rcp = eos_pool_flush(ctx, s)) return rcp;   // (the older calls first)
+    if (!ctx->eos_any) return 0;
     EosTab &E = ctx->eos_pending;
     if (ctx->pool_end > 0) {
-        k_eos_tab<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, on_comm_stream ? on_comm_stream : ctx->stream>>>(
+        k_eos_tab<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, s>>>(
             ctx->f64[B200SPH_RHO], f32_ptr(ctx, B200SPH_P), f32_ptr(ctx, B200SPH_CS), ctx->ptype, ctx->pool_end, E);
         LAUNCH_CHECK();
     }
@@ -1974,6 +2027,12 @@ static int ab_positions(b200sph_ctx *ctx)
 static int pack_state(b200sph_ctx *ctx)
 {
     if (int rc = ab_positions(ctx)) return rc;   // (k_pack_rec32 reads them)
+    // the packers read the pool's rho and apply eos_pending to it (eos_flush's order: the
+    // initialize, then the older calls)
+    if (ctx->eos_any || ctx->eos_pool_any) {
+        if (int rc = init_materialise(ctx)) return rc;
+        if (int rc = eos_pool_flush(ctx, ctx->stream)) return rc;
+    }
     if (ctx->rec32 && ctx->n_sorted > 0) {
         // (every particle is sorted: no ghosts, so the pool side of the EOS calls is complete)
         k_pack_rec32<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
@@ -2042,7 +2101,7 @@ static int arr_range(b200sph_ctx *ctx, int arr, int real_only, int64_t *lo, int6
 int b200sph_eos(b200sph_ctx *ctx, int arr, int hg, double rho0, double c0, double gamma, double p0, int real_only)
 {
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_pool(ctx, false);   // only book-keeping here: a halo in flight stays in flight
+    int rc = ensure_pool(ctx, false, true);   // only book-keeping here: a halo in flight stays in flight
     if (rc) return rc;
     if (arr < 0 || arr >= ctx->narr) return set_err(ctx, "bad array index %d", arr);
     EosTab &E = ctx->eos_pending;
@@ -2276,10 +2335,11 @@ static int records32(b200sph_ctx *ctx, const bool wcsph_list_pass, bool *yes, in
     return 0;
 }
 
+static bool can_fuse_stage(const b200sph_ctx *ctx, int arr);
 int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_t *pairs_out)
 {
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_pool(ctx, false);   // a halo in flight is waited for below, as late as possible
+    int rc = ensure_pool(ctx, false, true);   // a halo in flight is waited for below, as late as possible
     if (rc) return rc;
     if (!ctx->grid_valid) return set_err(ctx, "pair_pass: the NNPS is stale (particles were pushed/resized); call nnps_update first");
     if (ctx->spec_records && ctx->state_packed) {
@@ -2312,6 +2372,9 @@ int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_
     for (int d = 0; d < ctx->narr; d++)
         for (int sx = 0; sx < ctx->narr; sx++) prog_bits |= prog->eqmask[d][sx];
     const bool wcsph_only = !(prog_bits & ~(unsigned)PAIR_EQS_WCSPH) && !prog->tensile_correction;
+    // SummationDensity stores rho: a deferred initialize must have copied it before
+    const bool writes_rho = (prog_bits & B200SPH_EQ_SUMMATION_DENSITY) != 0;
+    if (writes_rho && (rc = init_materialise(ctx))) return rc;
     bool r32 = false;
     int ea = -1;
     if ((rc = records32(ctx, use_lists && !ranged && wcsph_only, &r32, &ea))) return rc;
@@ -2340,8 +2403,17 @@ int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_
     if (!overlap && (rc = sync_comm(ctx))) return rc;
     if (!ctx->state_packed) {
         if ((rc = pack_state(ctx))) return rc;
-    } else if (!overlap && (rc = eos_flush(ctx))) {   // the records have them; now the pool's rho / p / cs
-        return rc;
+    } else if (!overlap) {
+        // the records have the calls; the pool's rho / p / cs get them now or, when the next
+        // stage can be the fused kernel and this pass leaves rho alone, in that kernel
+        if (ctx->eos_any && !ctx->eos_pool_any && !writes_rho && !ctx->peer_box && can_fuse_stage(ctx, -1)) {
+            ctx->eos_pool = ctx->eos_pending;
+            ctx->eos_pool_any = true;
+            memset(ctx->eos_pending.on, 0, sizeof(ctx->eos_pending.on));
+            ctx->eos_any = false;
+        } else if ((ctx->eos_any || writes_rho) && (rc = eos_flush(ctx))) {
+            return rc;
+        }
     }
     if (!use_lists && (ctx->periodic[0] || ctx->periodic[1] || ctx->periodic[2]))
         return set_err(ctx, "periodic domains need the neighbour-list path (B200SPH_PAIR_KERNEL=list, < 2^26 particles)");
@@ -2645,11 +2717,11 @@ int b200sph_solid_pass(b200sph_ctx *ctx, const b200sph_solid_program *prog, int6
 static int ensure_tc(b200sph_ctx *ctx);
 // what every stage entry point (WCSPHStep, WCSPHTVDRK3Step, the EDAC steppers, SolidMechStep)
 // checks and prepares before it fills its arguments; `last` is the stepper's last stage
-static int stage_begin(b200sph_ctx *ctx, const char *who, int arr, int which, bool devdt, int last = 2)
+static int stage_begin(b200sph_ctx *ctx, const char *who, int arr, int which, bool devdt, int last = 2, bool keep_init = false)
 {
     if (int rcc = require_confirmed(ctx, who)) return rcc;
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_pool(ctx);
+    int rc = ensure_pool(ctx, true, keep_init);
     if (rc) return rc;
     if (arr >= ctx->narr) return set_err(ctx, "%s: bad array %d", who, arr);
     if (last == 3 && (which < 0 || which > 3))
@@ -2735,14 +2807,22 @@ static bool can_fuse_stage(const b200sph_ctx *ctx, int arr)
 static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devdt, bool rk3 = false)
 {
     const int last = rk3 ? 3 : 2;
-    int rc = stage_begin(ctx, rk3 ? "stage_rk3" : "stage", arr, which, devdt, last);
-    if (rc || (rc = eos_flush(ctx))) return rc;
+    int rc = stage_begin(ctx, rk3 ? "stage_rk3" : "stage", arr, which, devdt, last, true);
+    if (rc) return rc;
+    const bool fused = ctx->pool_end > 0 && can_fuse_stage(ctx, arr);
+    // EOS calls issued since the last pair pass, or any before an initialize (which copies the
+    // rho they clamp), go to the pool now; the pool side a pair pass left is the fused kernel's
+    if ((which == 0 || !fused || ctx->eos_any) && (rc = eos_flush(ctx))) return rc;
+    if (which == 0 && fused && !ctx->peer_box) {   // waits for the fused stage (init_materialise)
+        ctx->init_pending = true;
+        return 0;
+    }
     PhaseTimer pt(ctx, 2);
     StageArgs sa;
     stage_args(ctx, sa, arr, which, dt);
     if (rk3) sa.f = dt;   // every TVD-RK3 stage takes the whole dt
     sa.rho = ctx->f64[B200SPH_RHO]; sa.rho0 = ctx->f64[B200SPH_RHO0]; sa.arho = f32_ptr(ctx, B200SPH_ARHO);
-    if (which != 0 && ctx->pool_end > 0 && can_fuse_stage(ctx, arr)) {
+    if (which != 0 && fused) {
         // stage + records of the next evaluation (+ the dt factors after the last stage) in one pass
         FusePackArgs q;
         memset(&q, 0, sizeof(q));
@@ -2757,10 +2837,14 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
         q.dt_cfl = f32_ptr(ctx, B200SPH_DT_CFL); q.dt_force = f32_ptr(ctx, B200SPH_DT_FORCE);
         q.red = ctx->red;
         q.tc = devdt ? ctx->tc : nullptr;
-        q.do_init = 0;
+        q.do_init = ctx->init_pending ? 1 : 0;
         q.reduce_dt = (which == last && ctx->dt_adaptive_seen) ? 1 : 0;
         q.eos_any = ctx->eos_last_valid ? 1 : 0;
         q.E = ctx->eos_last;
+        q.eos_pool = ctx->eos_pool_any ? 1 : 0;
+        q.EP = ctx->eos_pool;
+        ctx->init_pending = false;
+        ctx->eos_pool_any = false;
         if (q.reduce_dt && !ctx->red_armed) {
             k_red_init<<<1, 32, 0, ctx->stream>>>(ctx->red);
             LAUNCH_CHECK();
@@ -2781,6 +2865,7 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
         ctx->spec_confirmed = 0;
         return 0;
     }
+    if ((rc = init_materialise(ctx))) return rc;
     if (ctx->pool_end > 0) {
         const unsigned nb = (unsigned)cdiv(ctx->pool_end, 256);
         if (rk3 && which != 0) {
@@ -3697,6 +3782,8 @@ int b200sph_drop_ghosts(b200sph_ctx *ctx, int arr)
 {
     if (arr < 0 || arr >= ctx->narr) return set_err(ctx, "drop_ghosts: bad array %d", arr);
     if (ctx->arr[arr].n != ctx->arr[arr].n_real) {
+        CU(cudaSetDevice(ctx->device));
+        if (int rci = init_materialise(ctx)) return rci;
         ctx->arr[arr].n = ctx->arr[arr].n_real;
         set_changed(ctx);
     }

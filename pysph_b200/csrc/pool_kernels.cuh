@@ -179,11 +179,46 @@ __device__ __forceinline__ void stage_body(const StageArgs &a)
     }
 }
 
+// TaitEOS.loop wc/basic.py:60-65 ; TaitEOSHGCorrection.loop wc/basic.py:118-126: the pending
+// equation-of-state calls on the pool (rho clamp of the HG variant, p, cs); same arithmetic as
+// k_pack_state.  eos_tab_eval is the arithmetic on one particle's rho (clamped in place; true
+// when it was); k_eos_tab, k_pack_rec32 and the fused stage kernels all call it.
+__device__ __forceinline__ bool eos_tab_applies(const EosTab &E, const uint8_t t)
+{
+    const int a = t & 7;
+    return E.on[a] && !(E.real_only[a] && (t & PT_GHOST));
+}
+__device__ __forceinline__ bool eos_tab_eval(const EosTab &E, const int a, double &r, float &p, float &cs)
+{
+    const double rho0 = E.rho0[a];
+    const bool clamp = E.hg[a] && r < rho0;
+    if (clamp) r = rho0;
+    const double ratio = r * (1.0 / rho0);
+    const double Bc = rho0 * E.c0[a] * E.c0[a] / E.gamma[a];
+{ double rg_, rh_; tait_powers(ratio, E.gamma[a], rg_, rh_);
+    p = (float)((E.hg[a] ? 0.0 : E.p0[a]) + Bc * (rg_ - 1.0));
+    cs = (float)(E.c0[a] * rh_); }
+    return clamp;
+}
+__device__ __forceinline__ void eos_tab_apply(double *__restrict__ rho, float *__restrict__ p, float *__restrict__ cs,
+                                              const uint8_t t, const long long g, const EosTab &E)
+{
+    if (!eos_tab_applies(E, t)) return;
+    double r = rho[g];
+    float pg, csg;
+    if (eos_tab_eval(E, t & 7, r, pg, csg)) rho[g] = r;
+    p[g] = pg;
+    cs[g] = csg;
+}
+
 // ---------------------------------------------------------------------------
 // The fused stage kernels of the WCSPH fast path (every array steps with WCSPHStep:
 // k_stage_pack, or with WCSPHTVDRK3Step: k_stage_pack_rk3; the neighbour lists of the current
 // build are reusable): in ONE pass over the pool, per real particle,
-//   [initialize (integrator_step.py:51-61) when it was deferred to here]
+//   [initialize (integrator_step.py:51-61) when it was deferred to here: the copies take the
+//    rho of before the EOS calls below, as the reference's initialize, which runs before them]
+//   [the pool side of the last evaluation's EOS calls (k_eos_tab's arithmetic) when the pair
+//    pass left it to here: rho clamp, p, cs -- ghosts included, as k_eos_tab]
 //   stage1 / stage2 (integrator_step.py:63-91), fp64, bitwise what k_stage computes
 //     (k_stage_pack_rk3: stage1 / stage2 / stage3, :118-168, bitwise what k_stage_rk3 computes)
 //   the packed pair records of the NEXT evaluation at the particle's sorted slot:
@@ -194,13 +229,13 @@ __device__ __forceinline__ void stage_body(const StageArgs &a)
 //   the drift of the build (max |x - x_build|^2, max (h - h_build)) into red_u32
 //   [the stepper's last stage: the adaptive-dt factors max dt_cfl, max dt_force, min h into
 //    red[9,11,12]]
-// It replaces k_stage + k_stage(initialize) + k_pack_pos_light + k_pack_state (+ k_reduce_dt):
-// five sweeps over the fp64 state become one.  Ghost particles are not stepped
+// It replaces k_stage(initialize) + k_eos_tab + k_stage + k_pack_pos_light + k_pack_state
+// (+ k_reduce_dt): six sweeps over the fp64 state become one.  Ghost particles are not stepped
 // (integrator_cython.mako:97-111) and their records are refreshed by the halo scatter.
 // ---------------------------------------------------------------------------
 struct FusePackArgs {
     const double *h, *m;
-    const float *p, *cs;             // pool values, used for arrays without a speculated EOS
+    float *p, *cs;                   // pool values: read for arrays without a speculated EOS, written by EP
     const uint32_t *rank, *key_of;   // pool index -> sorted slot / cell key of the current build
     const float4 *A0;                // packed positions at build time (sorted order)
     float4 *AB, *C;
@@ -213,17 +248,25 @@ struct FusePackArgs {
     const double *tc;                // device-resident dt (tc[0]); null: StageArgs.f
     int do_init, reduce_dt, eos_any;
     EosTab E;
+    int eos_pool;                    // apply EP to the pool's rho / p / cs first
+    EosTab EP;
 };
 
 // WCSPHTVDRK3Step.stage1 / stage2 / stage3 (integrator_step.py:118-168) for one property, in the
-// reference's association order; q is read by stages 2 and 3 only.  k_stage_rk3 and
-// k_stage_pack_rk3 both call it, so that both contract it to the same FMAs.
+// reference's association order (rk3_combine, on the current value qc); rk3_update reads q[g]
+// for stages 2 and 3 only.  k_stage_rk3 and k_stage_pack_rk3 both go through rk3_combine, so that
+// both contract it to the same FMAs (k_stage_pack_rk3 passes rho after the pool-side EOS clamp).
+__device__ __forceinline__ double rk3_combine(const int which, const double q0, const double qc, const double dt,
+                                              const float aq)
+{
+    if (which == 1) return q0 + dt * (double)aq;
+    if (which == 2) return 0.75 * q0 + 0.25 * (qc + dt * (double)aq);
+    return (1. / 3.) * q0 + (2. / 3.) * (qc + dt * (double)aq);
+}
 __device__ __forceinline__ double rk3_update(const int which, const double q0, const double *q,
                                              const long long g, const double dt, const float aq)
 {
-    if (which == 1) return q0 + dt * (double)aq;
-    if (which == 2) return 0.75 * q0 + 0.25 * (q[g] + dt * (double)aq);
-    return (1. / 3.) * q0 + (2. / 3.) * (q[g] + dt * (double)aq);
+    return rk3_combine(which, q0, which == 1 ? 0.0 : q[g], dt, aq);
 }
 
 // WCSPHTVDRK3Step stage1 / stage2 / stage3 (a.which = 1, 2, 3) with dt = a.f, real particles only;
@@ -264,17 +307,25 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
     if (t != PT_INVALID) {
         const double hg = q.h[g];
         hm = hg;
-        if (!(t & PT_GHOST)) {
+        if (t & PT_GHOST) {
+            if (q.eos_pool) eos_tab_apply(a.rho, q.p, q.cs, t, g, q.EP);
+        } else {
             double f = a.f;
             if (q.tc) {
                 const double dt = q.tc[0];
                 f = RK3 ? dt : (a.which == 1 ? 0.5 * dt : dt);
             }
+            // rho before the stage: the deferred initialize copies it as it is, the pool side of
+            // the EOS calls clamps it; the stage overwrites the pool's rho, so only TVD-RK3's
+            // stages 2 and 3 read the clamped value
+            const bool eos = q.eos_pool && eos_tab_applies(q.EP, t);
+            double rc = 0.0;
+            if (q.do_init || eos || (RK3 && a.which != 1)) rc = a.rho[g];
             double x0, y0, z0, u0, v0, w0, r0;
             if (q.do_init) {
                 x0 = a.x[g]; y0 = a.y[g]; z0 = a.z[g];
                 u0 = a.u[g]; v0 = a.v[g]; w0 = a.w[g];
-                r0 = a.rho[g];
+                r0 = rc;
                 a.x0[g] = x0; a.y0[g] = y0; a.z0[g] = z0;
                 a.u0[g] = u0; a.v0[g] = v0; a.w0[g] = w0;
                 a.rho0[g] = r0;
@@ -282,6 +333,12 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
                 x0 = a.x0[g]; y0 = a.y0[g]; z0 = a.z0[g];
                 u0 = a.u0[g]; v0 = a.v0[g]; w0 = a.w0[g];
                 r0 = a.rho0[g];
+            }
+            float p_eos = 0.f, cs_eos = 0.f;
+            if (eos) {
+                eos_tab_eval(q.EP, t & 7, rc, p_eos, cs_eos);
+                q.p[g] = p_eos;
+                q.cs[g] = cs_eos;
             }
             double un, vn, wn, xn, yn, zn, r;
             if (RK3) {
@@ -291,7 +348,7 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
                 xn = rk3_update(a.which, x0, a.x, g, f, a.ax[g]);
                 yn = rk3_update(a.which, y0, a.y, g, f, a.ay[g]);
                 zn = rk3_update(a.which, z0, a.z, g, f, a.az[g]);
-                r = rk3_update(a.which, r0, a.rho, g, f, a.arho[g]);
+                r = rk3_combine(a.which, r0, rc, f, a.arho[g]);
             } else {
                 un = u0 + f * (double)a.au[g];
                 vn = v0 + f * (double)a.av[g];
@@ -337,6 +394,9 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
 { double rg_, rh_; tait_powers(ratio, q.E.gamma[ar], rg_, rh_);
                     pg = (float)((q.E.hg[ar] ? 0.0 : q.E.p0[ar]) + Bc * (rg_ - 1.0));
                     csg = (float)(q.E.c0[ar] * rh_); }
+                } else if (eos) {
+                    pg = p_eos;
+                    csg = cs_eos;
                 } else {
                     pg = q.p[g];
                     csg = q.cs[g];
@@ -407,26 +467,6 @@ __global__ void __launch_bounds__(256, 4) k_stage_pack_rk3(const StageArgs a, co
     stage_pack_body<true>(a, q, s_d2, s_dh, s_mc, s_mf, s_hm);
 }
 
-// TaitEOS.loop wc/basic.py:60-65 ; TaitEOSHGCorrection.loop wc/basic.py:118-126: the pending
-// equation-of-state calls of every array in one launch (pool side: rho clamp of the HG
-// variant, p, cs); same arithmetic as k_pack_state
-__device__ __forceinline__ void eos_tab_apply(double *__restrict__ rho, float *__restrict__ p, float *__restrict__ cs,
-                                              const uint8_t t, const long long g, const EosTab &E)
-{
-    const int a = t & 7;
-    if (!E.on[a] || (E.real_only[a] && (t & PT_GHOST))) return;
-    double r = rho[g];
-    const double rho0 = E.rho0[a];
-    if (E.hg[a] && r < rho0) {
-        r = rho0;
-        rho[g] = r;
-    }
-    const double ratio = r * (1.0 / rho0);
-    const double Bc = rho0 * E.c0[a] * E.c0[a] / E.gamma[a];
-{ double rg_, rh_; tait_powers(ratio, E.gamma[a], rg_, rh_);
-    p[g] = (float)((E.hg[a] ? 0.0 : E.p0[a]) + Bc * (rg_ - 1.0));
-    cs[g] = (float)(E.c0[a] * rh_); }
-}
 __global__ void k_eos_tab(double *__restrict__ rho, float *__restrict__ p, float *__restrict__ cs,
                           const uint8_t *__restrict__ ptype, long long pool_end, const EosTab E)
 {
