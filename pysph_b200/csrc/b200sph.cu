@@ -113,6 +113,42 @@ __host__ __device__ static inline void grid_decode(const int zorder, const uint3
     }
 }
 
+// A = (x, y, z relative to the origin of the cell `key`, h): the packed position of the pair
+// records.  ONE function for every writer (the build, the light refresh, the fused stage kernel,
+// the ghost refresh), so that they all produce the same floats.
+__device__ __forceinline__ float4 pack_position(const GridDev &G, const uint32_t key, const double x, const double y,
+                                                const double z, const double h)
+{
+    uint32_t cx, cy, cz;
+    grid_decode(G.zorder, (uint32_t)G.nc[0], (uint32_t)G.nc[1], key, cx, cy, cz);
+    float4 a;
+    a.x = (float)(x - (G.xmin[0] + (double)cx * G.cell[0]));
+    a.y = (float)(y - (G.xmin[1] + (double)cy * G.cell[1]));
+    a.z = (float)(z - (G.xmin[2] + (double)cz * G.cell[2]));
+    a.w = (float)h;
+    return a;
+}
+
+// how far the packed position A has drifted from A0, its value at the build:
+// d2 = |A - A0|^2, dh = max(h - h_build, 0)
+__device__ __forceinline__ void build_drift(const float4 A, const float4 A0, float &d2, float &dh)
+{
+    const float dx = A.x - A0.x, dy = A.y - A0.y, dz = A.z - A0.z;
+    d2 = dx * dx + dy * dy + dz * dz;
+    dh = fmaxf(A.w - A0.w, 0.f);
+}
+
+// The factor of dt a stage steps by.  With the device-resident dt (tc not null) it is formed
+// here from tc[0]: dt / 2 in stage1 of WCSPHStep (and of EDACStep, EDACTVFStep, SolidMechStep),
+// dt in their stage2 and in every stage of WCSPHTVDRK3Step (whole); otherwise it is the host's
+// factor f.  Every stage kernel, fused or not, takes its factor from here.
+__device__ __forceinline__ double stage_factor(const double *tc, const double f, const int which, const bool whole)
+{
+    if (!tc) return f;
+    const double dt = tc[0];
+    return whole || which != 1 ? dt : 0.5 * dt;
+}
+
 // equation-of-state calls wait here until the next k_pack_state applies them in the
 // same pass that gathers the state into the pair records (saves one launch and one
 // sweep over rho/p/cs per array and evaluation); eos_flush() runs them stand-alone
@@ -137,6 +173,41 @@ __host__ __device__ static inline void tait_powers(const double ratio, const dou
         rg = pow(ratio, gamma);
         rh = pow(ratio, 0.5 * (gamma - 1.0));
     }
+}
+
+// TaitEOS.loop wc/basic.py:60-65 ; TaitEOSHGCorrection.loop wc/basic.py:118-126 on one particle
+// of array a: the rho clamp of the HG variant (r clamped in place; true when it was), p and cs.
+// The one evaluation of the EOS: every kernel that applies it calls this, and decides itself
+// whether the clamped rho goes back to the pool or stays in its record.
+__device__ __forceinline__ bool eos_tab_applies(const EosTab &E, const uint8_t t)
+{
+    const int a = t & 7;
+    return E.on[a] && !(E.real_only[a] && (t & PT_GHOST));
+}
+__device__ __forceinline__ bool eos_tab_eval(const EosTab &E, const int a, double &r, float &p, float &cs)
+{
+    const double rho0 = E.rho0[a];
+    const bool clamp = E.hg[a] && r < rho0;
+    if (clamp) r = rho0;
+    const double ratio = r * (1.0 / rho0);
+    const double Bc = rho0 * E.c0[a] * E.c0[a] / E.gamma[a];
+    double rg, rh;
+    tait_powers(ratio, E.gamma[a], rg, rh);
+    p = (float)((E.hg[a] ? 0.0 : E.p0[a]) + Bc * (rg - 1.0));
+    cs = (float)(E.c0[a] * rh);
+    return clamp;
+}
+
+// B = (u, v, w, m), C = (rho, p / rho^2, cs, type): the state half of the 48-byte pair records.
+// ONE function for every writer, so that they all produce the same floats.
+__device__ __forceinline__ void state_record(const double u, const double v, const double w, const double m, const double r,
+                                             const float p, const float cs, const int t, float4 &B, float4 &C)
+{
+    B.x = (float)u; B.y = (float)v; B.z = (float)w; B.w = (float)m;
+    C.x = (float)r;
+    C.y = (float)((double)p / (r * r));
+    C.z = cs;
+    C.w = __int_as_float(t);
 }
 
 // The one Tait EOS (gamma = 7) the 32-byte records are formed with: rho0, B = rho0 c0^2 / 7 and
@@ -879,8 +950,9 @@ template <class F> static int with_halo_fields(const b200sph_ctx *ctx, F &&launc
     return launch(std::integral_constant<int, B200SPH_HALO_FIELDS_SOLID>());
 }
 
-// the fields StageArgs, StageTvfArgs and StageSolidArgs have in common, by name
-template <class S> static void stage_args(b200sph_ctx *ctx, S &sa, int arr, int which, double dt)
+// the fields StageArgs, StageTvfArgs and StageSolidArgs have in common, by name (devdt: the
+// kernel takes dt from the time-control block)
+template <class S> static void stage_args(b200sph_ctx *ctx, S &sa, int arr, int which, double dt, bool devdt)
 {
     sa.x = ctx->f64[B200SPH_X]; sa.y = ctx->f64[B200SPH_Y]; sa.z = ctx->f64[B200SPH_Z];
     sa.u = ctx->f64[B200SPH_U]; sa.v = ctx->f64[B200SPH_V]; sa.w = ctx->f64[B200SPH_W];
@@ -893,6 +965,7 @@ template <class S> static void stage_args(b200sph_ctx *ctx, S &sa, int arr, int 
     sa.arr = arr;
     sa.which = which;
     sa.f = which == 1 ? 0.5 * dt : dt;
+    sa.tc = devdt ? ctx->tc : nullptr;
 }
 
 // ---- the deferred initialize ----------------------------------------------------------------
@@ -908,7 +981,7 @@ static int init_materialise(b200sph_ctx *ctx)
     if (!ctx->init_pending) return 0;
     ctx->init_pending = false;
     StageArgs sa;
-    stage_args(ctx, sa, -1, 0, 0.0);
+    stage_args(ctx, sa, -1, 0, 0.0, false);
     sa.rho = ctx->f64[B200SPH_RHO]; sa.rho0 = ctx->f64[B200SPH_RHO0]; sa.arho = f32_ptr(ctx, B200SPH_ARHO);
     if (ctx->pool_end > 0) {
         k_stage<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
@@ -1557,6 +1630,20 @@ static bool retire_build(b200sph_ctx *ctx)
     return false;
 }
 
+// k_pack_pos_light: the packed positions refreshed in the frozen order of the build, their drift
+// since the build max-reduced into red_u32[0..1] after the first `clear` words of red_u32 are
+// zeroed (0: the drift is added to what red_u32 holds)
+static int pack_positions_light(b200sph_ctx *ctx, int clear)
+{
+    if (clear) CU(cudaMemsetAsync(ctx->red_u32, 0, clear * sizeof(unsigned), ctx->stream));
+    k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
+        ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H], ctx->perm, ctx->skey,
+        ctx->n_sorted, ctx->G, ctx->A0, ctx->A, ctx->AB, ctx->red_u32);
+    ctx->ab_stale = false;   // (k_pack_pos_light writes the position half of AB)
+    LAUNCH_CHECK();
+    return 0;
+}
+
 // light path of nnps_update: same sorted order, same cell frames, fresh positions;
 // returns 1 if the persistent lists are still valid, 0 if a full rebuild is needed
 static int nnps_light_update(b200sph_ctx *ctx)
@@ -1568,20 +1655,11 @@ static int nnps_light_update(b200sph_ctx *ctx)
         ctx->drift_ok = false;
         drift_consumed(ctx);
         if (ctx->packed_valid) return 1;   // nnps_drift_device packed them, halo_overwrite_all kept the ghosts current
-        k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
-            ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H], ctx->perm, ctx->skey,
-            ctx->n_sorted, ctx->G, ctx->A0, ctx->A, ctx->AB, ctx->red_u32);
-        ctx->ab_stale = false;   // (k_pack_pos_light writes the position half of AB)
-        LAUNCH_CHECK();
+        if (int rc = pack_positions_light(ctx, 0)) return rc;
         return 1;
     }
     if (!(ctx->packed_valid && ctx->drift_measured)) {   // (the fused stage kernel packs and measures)
-        CU(cudaMemsetAsync(ctx->red_u32, 0, 4 * sizeof(unsigned), ctx->stream));
-        k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
-            ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H], ctx->perm, ctx->skey,
-            ctx->n_sorted, ctx->G, ctx->A0, ctx->A, ctx->AB, ctx->red_u32);
-        ctx->ab_stale = false;   // (k_pack_pos_light writes the position half of AB)
-        LAUNCH_CHECK();
+        if (int rc = pack_positions_light(ctx, 4)) return rc;
     }
     drift_consumed(ctx);
     ctx->packed_valid = true;
@@ -2737,7 +2815,7 @@ static int stage_solid_impl(b200sph_ctx *ctx, int arr, int which, double dt, boo
     if (rc || (rc = ensure_solid(ctx))) return rc;
     PhaseTimer pt(ctx, 2);
     StageSolidArgs sa;
-    stage_args(ctx, sa, arr, which, dt);
+    stage_args(ctx, sa, arr, which, dt, devdt);
     sa.rho = ctx->f64[B200SPH_RHO]; sa.rho0 = ctx->f64[B200SPH_RHO0]; sa.arho = f32_ptr(ctx, B200SPH_ARHO);
     for (int k = 0; k < 6; k++) {
         sa.s[k] = ctx->f64s[k];
@@ -2745,8 +2823,7 @@ static int stage_solid_impl(b200sph_ctx *ctx, int arr, int which, double dt, boo
         sa.as[k] = ctx->f32s[15 + k];
     }
     if (ctx->pool_end > 0) {
-        if (devdt) k_stage_solid_devdt<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa, ctx->tc);
-        else k_stage_solid<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
+        k_stage_solid<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
         LAUNCH_CHECK();
     }
     if (which != 0) particles_moved(ctx);
@@ -2761,15 +2838,14 @@ static int stage_tvf_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool 
     if (rc) return rc;
     PhaseTimer pt(ctx, 2);
     StageTvfArgs sa;
-    stage_args(ctx, sa, arr, which, dt);
+    stage_args(ctx, sa, arr, which, dt, devdt);
     sa.uh = f64_ptr(ctx, B200SPH_UHAT); sa.vh = f64_ptr(ctx, B200SPH_VHAT); sa.wh = f64_ptr(ctx, B200SPH_WHAT);
     sa.pf = f64_ptr(ctx, B200SPH_PF); sa.pf0 = f64_ptr(ctx, B200SPH_PF0);
     sa.auh = f32_ptr(ctx, B200SPH_AUHAT); sa.avh = f32_ptr(ctx, B200SPH_AVHAT);
     sa.awh = f32_ptr(ctx, B200SPH_AWHAT); sa.ap = f32_ptr(ctx, B200SPH_AP);
     sa.ext = ext;
     if (ctx->pool_end > 0) {
-        if (devdt) k_stage_tvf_devdt<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa, ctx->tc);
-        else k_stage_tvf<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
+        k_stage_tvf<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
         LAUNCH_CHECK();
     }
     if (which != 0) particles_moved(ctx);
@@ -2819,7 +2895,7 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
     }
     PhaseTimer pt(ctx, 2);
     StageArgs sa;
-    stage_args(ctx, sa, arr, which, dt);
+    stage_args(ctx, sa, arr, which, dt, devdt);
     if (rk3) sa.f = dt;   // every TVD-RK3 stage takes the whole dt
     sa.rho = ctx->f64[B200SPH_RHO]; sa.rho0 = ctx->f64[B200SPH_RHO0]; sa.arho = f32_ptr(ctx, B200SPH_ARHO);
     if (which != 0 && fused) {
@@ -2836,7 +2912,6 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
         q.red_u32 = ctx->red_u32;
         q.dt_cfl = f32_ptr(ctx, B200SPH_DT_CFL); q.dt_force = f32_ptr(ctx, B200SPH_DT_FORCE);
         q.red = ctx->red;
-        q.tc = devdt ? ctx->tc : nullptr;
         q.do_init = ctx->init_pending ? 1 : 0;
         q.reduce_dt = (which == last && ctx->dt_adaptive_seen) ? 1 : 0;
         q.eos_any = ctx->eos_last_valid ? 1 : 0;
@@ -2868,10 +2943,7 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
     if ((rc = init_materialise(ctx))) return rc;
     if (ctx->pool_end > 0) {
         const unsigned nb = (unsigned)cdiv(ctx->pool_end, 256);
-        if (rk3 && which != 0) {
-            if (devdt) k_stage_rk3_devdt<<<nb, 256, 0, ctx->stream>>>(sa, ctx->tc);
-            else k_stage_rk3<<<nb, 256, 0, ctx->stream>>>(sa);
-        } else if (devdt) k_stage_devdt<<<nb, 256, 0, ctx->stream>>>(sa, ctx->tc);
+        if (rk3 && which != 0) k_stage_rk3<<<nb, 256, 0, ctx->stream>>>(sa);
         else k_stage<<<nb, 256, 0, ctx->stream>>>(sa);
         LAUNCH_CHECK();
     }
@@ -3290,14 +3362,7 @@ int b200sph_nnps_drift(b200sph_ctx *ctx, double out[2])
     if (!reusable_build(ctx)) return 0;
     if (retire_build(ctx)) return 0;
     if (ctx->n_sorted <= 0) { out[0] = 0.0; return 0; }
-    if (!(ctx->packed_valid && ctx->drift_measured)) {
-        CU(cudaMemsetAsync(ctx->red_u32, 0, 2 * sizeof(unsigned), ctx->stream));
-        k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
-            ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H], ctx->perm, ctx->skey,
-            ctx->n_sorted, ctx->G, ctx->A0, ctx->A, ctx->AB, ctx->red_u32);
-        ctx->ab_stale = false;   // (k_pack_pos_light writes the position half of AB)
-        LAUNCH_CHECK();
-    }
+    if (!(ctx->packed_valid && ctx->drift_measured) && (rc = pack_positions_light(ctx, 2))) return rc;
     CU(cudaMemcpyAsync(ctx->red_u32_host, ctx->red_u32, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
     float d2, dh;
@@ -3333,23 +3398,31 @@ int b200sph_halo_pack_selected_all(b200sph_ctx *ctx, int slot, double *dev_buf, 
     });
 }
 
+// the ghost ranges [ghost_first[a], ghost_first[a] + counts[a]) of every array, checked against
+// the array's ghosts, as the scatter's HaloAllArgs
+static int ghost_ranges(b200sph_ctx *ctx, const char *who, const int64_t *ghost_first, const int64_t *counts, HaloAllArgs &A)
+{
+    A.narr = ctx->narr;
+    A.prefix[0] = 0;
+    for (int a = 0; a < ctx->narr; a++) {
+        const ArrayInfo &ai = ctx->arr[a];
+        if (ghost_first[a] < 0 || counts[a] < 0 || ai.n_real + ghost_first[a] + counts[a] > ai.n)
+            return set_err(ctx, "%s: ghosts [%lld, %lld) outside the %lld ghosts of '%s'", who, (long long)ghost_first[a],
+                           (long long)(ghost_first[a] + counts[a]), (long long)(ai.n - ai.n_real), ai.name.c_str());
+        A.prefix[a + 1] = A.prefix[a] + counts[a];
+        A.off[a] = ai.off + ai.n_real + ghost_first[a];
+        A.idx[a] = nullptr;
+    }
+    return 0;
+}
+
 int b200sph_halo_overwrite_all(b200sph_ctx *ctx, const int64_t *ghost_first, const int64_t *counts, const double *dev_buf)
 {
     CU(cudaSetDevice(ctx->device));
     int rc = ensure_pool(ctx);
     if (rc) return rc;
     HaloAllArgs A;
-    A.narr = ctx->narr;
-    A.prefix[0] = 0;
-    for (int a = 0; a < ctx->narr; a++) {
-        const ArrayInfo &ai = ctx->arr[a];
-        if (ghost_first[a] < 0 || counts[a] < 0 || ai.n_real + ghost_first[a] + counts[a] > ai.n)
-            return set_err(ctx, "halo_overwrite_all: ghosts [%lld, %lld) outside the %lld ghosts of '%s'", (long long)ghost_first[a],
-                           (long long)(ghost_first[a] + counts[a]), (long long)(ai.n - ai.n_real), ai.name.c_str());
-        A.prefix[a + 1] = A.prefix[a] + counts[a];
-        A.off[a] = ai.off + ai.n_real + ghost_first[a];
-        A.idx[a] = nullptr;
-    }
+    if ((rc = ghost_ranges(ctx, "halo_overwrite_all", ghost_first, counts, A))) return rc;
     const int64_t tot = A.prefix[ctx->narr];
     if (tot == 0) return 0;
     // with a reusable build whose packed positions are current (nnps_drift_device just
@@ -3419,14 +3492,7 @@ int b200sph_nnps_drift_device(b200sph_ctx *ctx, double *dev_ratio)
         CU(cudaMemsetAsync(dev_ratio, 0, sizeof(double), ctx->stream));
         return 0;
     }
-    if (!(ctx->packed_valid && ctx->drift_measured)) {   // (the fused stage kernel packs and measures)
-        CU(cudaMemsetAsync(ctx->red_u32, 0, 2 * sizeof(unsigned), ctx->stream));
-        k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
-            ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H], ctx->perm, ctx->skey,
-            ctx->n_sorted, ctx->G, ctx->A0, ctx->A, ctx->AB, ctx->red_u32);
-        ctx->ab_stale = false;   // (k_pack_pos_light writes the position half of AB)
-        LAUNCH_CHECK();
-    }
+    if (!(ctx->packed_valid && ctx->drift_measured) && (rc = pack_positions_light(ctx, 2))) return rc;   // (the fused stage kernel packs and measures)
     k_drift_ratio<<<1, 1, 0, ctx->stream>>>(ctx->red_u32, (float)ctx->radius_scale, (float)ctx->S_abs, dev_ratio);
     LAUNCH_CHECK();
     ctx->packed_valid = true;
@@ -3534,14 +3600,8 @@ int b200sph_peer_begin(b200sph_ctx *ctx)
     if (!ctx->peer_connected) return set_err(ctx, "peer_begin: the mailboxes are not connected");
     if ((rc = eos_flush(ctx))) return rc;
     const int no_build = !reusable_build(ctx) || retire_build(ctx);
-    if (!no_build && ctx->n_sorted > 0 && !(ctx->packed_valid && ctx->drift_measured)) {
-        CU(cudaMemsetAsync(ctx->red_u32, 0, 2 * sizeof(unsigned), ctx->stream));
-        k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
-            ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H], ctx->perm, ctx->skey,
-            ctx->n_sorted, ctx->G, ctx->A0, ctx->A, ctx->AB, ctx->red_u32);
-        ctx->ab_stale = false;   // (k_pack_pos_light writes the position half of AB)
-        LAUNCH_CHECK();
-    }
+    if (!no_build && ctx->n_sorted > 0 && !(ctx->packed_valid && ctx->drift_measured) && (rc = pack_positions_light(ctx, 2)))
+        return rc;
     if (!no_build) ctx->packed_valid = true, ctx->drift_measured = true;
     ctx->peer_epoch++;
     CU(cudaEventRecord(ctx->ev_fork, ctx->stream));
@@ -3672,17 +3732,7 @@ int b200sph_peer_recv(b200sph_ctx *ctx, int side, const int64_t *ghost_first, co
     if (!ctx->peer_connected) return set_err(ctx, "peer_recv: the mailboxes are not connected");
     if (side < 0 || side > 1) return set_err(ctx, "peer_recv: bad side");
     HaloAllArgs A;
-    A.narr = ctx->narr;
-    A.prefix[0] = 0;
-    for (int a = 0; a < ctx->narr; a++) {
-        const ArrayInfo &ai = ctx->arr[a];
-        if (ghost_first[a] < 0 || counts[a] < 0 || ai.n_real + ghost_first[a] + counts[a] > ai.n)
-            return set_err(ctx, "peer_recv: ghosts [%lld, %lld) outside the %lld ghosts of '%s'", (long long)ghost_first[a],
-                           (long long)(ghost_first[a] + counts[a]), (long long)(ai.n - ai.n_real), ai.name.c_str());
-        A.prefix[a + 1] = A.prefix[a] + counts[a];
-        A.off[a] = ai.off + ai.n_real + ghost_first[a];
-        A.idx[a] = nullptr;
-    }
+    if (int rc = ghost_ranges(ctx, "peer_recv", ghost_first, counts, A)) return rc;
     const int64_t tot = A.prefix[ctx->narr];
     if (tot == 0) return 0;
     int rc = refresh_ptype(ctx);

@@ -164,14 +164,7 @@ __global__ void k_halo_scatter_all(HaloPtrs P, HaloAllArgs A, const double *__re
     if (NF != B200SPH_HALO_FIELDS) P.cs[A.off[a] + r] = (float)in[(long long)(NF - 1) * cnt];
     if (R.rank) {
         const uint32_t s = R.rank[A.off[a] + r];
-        uint32_t key = R.skey[s];
-        uint32_t cx, cy, cz;
-        grid_decode(R.G.zorder, (uint32_t)R.G.nc[0], (uint32_t)R.G.nc[1], key, cx, cy, cz);
-        float4 q;
-        q.x = (float)(v[0] - (R.G.xmin[0] + (double)cx * R.G.cell[0]));
-        q.y = (float)(v[1] - (R.G.xmin[1] + (double)cy * R.G.cell[1]));
-        q.z = (float)(v[2] - (R.G.xmin[2] + (double)cz * R.G.cell[2]));
-        q.w = (float)v[7];
+        const float4 q = pack_position(R.G, R.skey[s], v[0], v[1], v[2], v[7]);
         R.A[s] = q;
         R.AB[2 * s] = q;
     }
@@ -389,7 +382,7 @@ __global__ void __launch_bounds__(PEER_NT) k_peer_push(HaloPtrs P, PeerPushArgs 
 
 // the packed pair records of a ghost, written by the receiving kernel (the fused stage
 // kernel only packs real particles): {A, B} at its sorted slot and C with the equation of
-// state that the last evaluation applied to ghosts (k_pack_state's arithmetic)
+// state that the last evaluation applied to ghosts (eos_tab_eval, state_record)
 struct GhostPackArgs {
     const uint32_t *rank, *skey;   // rank == nullptr: no records (no reusable build)
     float4 *A, *AB, *C;            // C == nullptr: positions only
@@ -441,14 +434,7 @@ __global__ void __launch_bounds__(PEER_NT) k_peer_pull(HaloPtrs P, PeerPullArgs 
     if (NF != B200SPH_HALO_FIELDS) P.cs[g] = (float)__ldcg(in + (long long)(NF - 1) * cnt);
     if (R.rank) {
         const uint32_t s = R.rank[g];
-        uint32_t key = R.skey[s];
-        uint32_t cx, cy, cz;
-        grid_decode(R.G.zorder, (uint32_t)R.G.nc[0], (uint32_t)R.G.nc[1], key, cx, cy, cz);
-        float4 q;
-        q.x = (float)(v[0] - (R.G.xmin[0] + (double)cx * R.G.cell[0]));
-        q.y = (float)(v[1] - (R.G.xmin[1] + (double)cy * R.G.cell[1]));
-        q.z = (float)(v[2] - (R.G.xmin[2] + (double)cz * R.G.cell[2]));
-        q.w = (float)v[7];
+        const float4 q = pack_position(R.G, R.skey[s], v[0], v[1], v[2], v[7]);
         R.A[s] = q;
         R.AB[2 * (size_t)s] = q;
         if (R.C) {
@@ -458,23 +444,13 @@ __global__ void __launch_bounds__(PEER_NT) k_peer_pull(HaloPtrs P, PeerPullArgs 
             double rr = v[6];
             float pg, csg;
             if (R.eos_any && R.E.on[ar] && !R.E.real_only[ar]) {
-                const double rho0 = R.E.rho0[ar];
-                if (R.E.hg[ar] && rr < rho0) rr = rho0;   // the record only; the pool side follows with the EOS calls
-                const double ratio = rr * (1.0 / rho0);
-                const double Bc = rho0 * R.E.c0[ar] * R.E.c0[ar] / R.E.gamma[ar];
-{ double rg_, rh_; tait_powers(ratio, R.E.gamma[ar], rg_, rh_);
-                pg = (float)((R.E.hg[ar] ? 0.0 : R.E.p0[ar]) + Bc * (rg_ - 1.0));
-                csg = (float)(R.E.c0[ar] * rh_); }
+                eos_tab_eval(R.E, ar, rr, pg, csg);   // the record only; the pool side follows with the EOS calls
             } else {
                 pg = R.p[g];
                 csg = R.cs[g];
             }
             float4 b, c;
-            b.x = (float)v[3]; b.y = (float)v[4]; b.z = (float)v[5]; b.w = (float)v[8];
-            c.x = (float)rr;
-            c.y = (float)((double)pg / (rr * rr));
-            c.z = csg;
-            c.w = __int_as_float(t);
+            state_record(v[3], v[4], v[5], v[8], rr, pg, csg, t, b, c);
             R.AB[2 * (size_t)s + 1] = b;
             R.C[s] = c;
         }

@@ -70,14 +70,7 @@ __global__ void k_pack_pos(const double *__restrict__ x, const double *__restric
     if (s >= n) return;
     const uint32_t g = perm[s];
     if (stype) stype[s] = ptype[g];
-    uint32_t key = skey[s];
-    uint32_t cx, cy, cz;
-    grid_decode(G.zorder, (uint32_t)G.nc[0], (uint32_t)G.nc[1], key, cx, cy, cz);
-    float4 a;
-    a.x = (float)(x[g] - (G.xmin[0] + (double)cx * G.cell[0]));
-    a.y = (float)(y[g] - (G.xmin[1] + (double)cy * G.cell[1]));
-    a.z = (float)(z[g] - (G.xmin[2] + (double)cz * G.cell[2]));
-    a.w = (float)h[g];
+    const float4 a = pack_position(G, skey[s], x[g], y[g], z[g], h[g]);
     A[s] = a;
     AB[2 * s] = a;
 }
@@ -96,32 +89,18 @@ __global__ void k_pack_state(const double *__restrict__ u, const double *__restr
     if (s >= n) return;
     const uint32_t g = perm[s];
     const int t = (int)ptype[g];
-    float4 b, c;
-    b.x = (float)u[g]; b.y = (float)v[g]; b.z = (float)w[g]; b.w = (float)m[g];
     double r = rho[g];
     float pg, csg;
-    const int a = t & 7;
-    if (eos_any && E.on[a] && !(E.real_only[a] && (t & PT_GHOST))) {
-        const double rho0 = E.rho0[a];
-        if (E.hg[a] && r < rho0) {
-            r = rho0;
-            rho[g] = r;
-        }
-        const double ratio = r * (1.0 / rho0);
-        const double Bc = rho0 * E.c0[a] * E.c0[a] / E.gamma[a];
-{ double rg_, rh_; tait_powers(ratio, E.gamma[a], rg_, rh_);
-        pg = (float)((E.hg[a] ? 0.0 : E.p0[a]) + Bc * (rg_ - 1.0));
-        csg = (float)(E.c0[a] * rh_); }
+    if (eos_any && eos_tab_applies(E, (uint8_t)t)) {
+        if (eos_tab_eval(E, t & 7, r, pg, csg)) rho[g] = r;
         p[g] = pg;
         cs[g] = csg;
     } else {
         pg = p[g];
         csg = cs[g];
     }
-    c.x = (float)r;
-    c.y = (float)((double)pg / (r * r));
-    c.z = csg;
-    c.w = __int_as_float(t);
+    float4 b, c;
+    state_record(u[g], v[g], w[g], m[g], r, pg, csg, t, b, c);
     B[s] = b;
     C[s] = c;
     AB[2 * s + 1] = b;

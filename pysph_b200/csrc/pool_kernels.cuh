@@ -91,7 +91,7 @@ __global__ void k_reduce_dt(const float *__restrict__ dt_cfl, const float *__res
 
 // Integrator.compute_time_step (integrator.py:161-200) on the reduced factors: the local
 // proposal cfl * dt_min, or 1e20 when no factor constrains it (solver.py:655-660)
-__global__ void k_dt_propose(long long *__restrict__ red, double *__restrict__ tc, double cfl, int fixed_h)
+__device__ __forceinline__ void dt_propose(const long long *red, double *tc, const double cfl, const int fixed_h)
 {
     const double mc = o2d(red[9]), mf = o2d(red[11]);
     const double f_cfl = mc < -1e299 ? -1.0 : mc, f_force = mf < -1e299 ? -1.0 : mf;
@@ -104,13 +104,11 @@ __global__ void k_dt_propose(long long *__restrict__ red, double *__restrict__ t
     if (f_force > 0.0) dt_force = sqrt(hmin / sqrt(f_force));
     const double dt_min = fmin(dt_cfl, dt_force);
     tc[2] = (dt_min <= 0.0 || isinf(dt_min)) ? 1e20 : cfl * dt_min;
-    // re-arm the slots for the next reduction (the fused stage kernel adds to them directly)
-    red[9] = d2o(-1e300); red[11] = d2o(-1e300); red[12] = d2o(1e300);
 }
 // Solver loop bookkeeping (solver.py:478-491, :647-688): t += dt; dt = damp(new dt)
 // and the last step lands on the final time (solver.py:757-760, :771-773)
-__global__ void k_dt_commit(double *__restrict__ tc, double prev_factor, double new_factor, int in_parallel, int adaptive, int advance,
-                            double t_final, double t_eps)
+__device__ __forceinline__ void dt_commit(double *tc, const double prev_factor, const double new_factor, const int in_parallel,
+                                          const int adaptive, const int advance, const double t_final, const double t_eps)
 {
     const double dt_old = tc[0];
     if (advance) tc[1] += dt_old;
@@ -125,6 +123,25 @@ __global__ void k_dt_commit(double *__restrict__ tc, double prev_factor, double 
     dt *= new_factor;
     if (t + dt > t_final - t_eps) dt = t_final - t;
     tc[0] = dt;
+}
+// the slots are re-armed for the next reduction (the fused stage kernel adds to them directly)
+__global__ void k_dt_propose(long long *__restrict__ red, double *__restrict__ tc, double cfl, int fixed_h)
+{
+    dt_propose(red, tc, cfl, fixed_h);
+    red[9] = d2o(-1e300); red[11] = d2o(-1e300); red[12] = d2o(1e300);
+}
+__global__ void k_dt_commit(double *__restrict__ tc, double prev_factor, double new_factor, int in_parallel, int adaptive, int advance,
+                            double t_final, double t_eps)
+{
+    dt_commit(tc, prev_factor, new_factor, in_parallel, adaptive, advance, t_final, t_eps);
+}
+// both in one launch (one rank: nothing to reduce in between)
+__global__ void k_dt_advance(long long *__restrict__ red, double *__restrict__ tc, double cfl, int fixed_h,
+                             double prev_factor, double new_factor, int adaptive, int advance, double t_final, double t_eps)
+{
+    if (adaptive) dt_propose(red, tc, cfl, fixed_h);
+    red[9] = d2o(-1e300); red[11] = d2o(-1e300); red[12] = d2o(1e300);
+    dt_commit(tc, prev_factor, new_factor, 0, adaptive, advance, t_final, t_eps);
 }
 // UpdateSmoothingLengthFerrari.loop wc/basic.py:458-463
 __global__ void k_ferrari(double *__restrict__ h, const double *__restrict__ m,
@@ -144,18 +161,34 @@ struct StageArgs {
     long long pool_end;
     int arr, which;
     double f;
+    const double *tc;                // device-resident dt (tc[0]); null: f
 };
+
+// WCSPHStep.stage1 / stage2 (integrator_step.py:63-91) for one property.  k_stage and
+// k_stage_pack both go through wcsph_combine, so that both contract it to the same FMA.
+__device__ __forceinline__ double wcsph_combine(const double q0, const double f, const float aq)
+{
+    return q0 + f * (double)aq;
+}
+// WCSPHTVDRK3Step.stage1 / stage2 / stage3 (integrator_step.py:118-168) for one property, in the
+// reference's association order (rk3_combine, on the current value qc); rk3_update reads q[g]
+// for stages 2 and 3 only.  k_stage_rk3 and k_stage_pack_rk3 both go through rk3_combine, so that
+// both contract it to the same FMAs (k_stage_pack_rk3 passes rho after the pool-side EOS clamp).
+__device__ __forceinline__ double rk3_combine(const int which, const double q0, const double qc, const double dt,
+                                              const float aq)
+{
+    if (which == 1) return q0 + dt * (double)aq;
+    if (which == 2) return 0.75 * q0 + 0.25 * (qc + dt * (double)aq);
+    return (1. / 3.) * q0 + (2. / 3.) * (qc + dt * (double)aq);
+}
+__device__ __forceinline__ double rk3_update(const int which, const double q0, const double *q,
+                                             const long long g, const double dt, const float aq)
+{
+    return rk3_combine(which, q0, which == 1 ? 0.0 : q[g], dt, aq);
+}
 
 // WCSPHStep.initialize / stage1 / stage2 integrator_step.py:51-91 (real particles only,
 // integrator_cython.mako:97-111)
-__device__ __forceinline__ void stage_body(const StageArgs &a);
-__global__ void k_stage(StageArgs a) { stage_body(a); }
-__global__ void k_stage_devdt(StageArgs a, const double *__restrict__ tc)
-{
-    const double dt = tc[0];
-    a.f = a.which == 1 ? 0.5 * dt : dt;
-    stage_body(a);
-}
 __device__ __forceinline__ void stage_body(const StageArgs &a)
 {
     long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -168,38 +201,39 @@ __device__ __forceinline__ void stage_body(const StageArgs &a)
         a.u0[g] = a.u[g]; a.v0[g] = a.v[g]; a.w0[g] = a.w[g];
         a.rho0[g] = a.rho[g];
     } else {
-        const double f = a.f;
-        a.u[g] = a.u0[g] + f * (double)a.au[g];
-        a.v[g] = a.v0[g] + f * (double)a.av[g];
-        a.w[g] = a.w0[g] + f * (double)a.aw[g];
-        a.x[g] = a.x0[g] + f * (double)a.ax[g];
-        a.y[g] = a.y0[g] + f * (double)a.ay[g];
-        a.z[g] = a.z0[g] + f * (double)a.az[g];
-        a.rho[g] = a.rho0[g] + f * (double)a.arho[g];
+        const double f = stage_factor(a.tc, a.f, a.which, false);
+        a.u[g] = wcsph_combine(a.u0[g], f, a.au[g]);
+        a.v[g] = wcsph_combine(a.v0[g], f, a.av[g]);
+        a.w[g] = wcsph_combine(a.w0[g], f, a.aw[g]);
+        a.x[g] = wcsph_combine(a.x0[g], f, a.ax[g]);
+        a.y[g] = wcsph_combine(a.y0[g], f, a.ay[g]);
+        a.z[g] = wcsph_combine(a.z0[g], f, a.az[g]);
+        a.rho[g] = wcsph_combine(a.rho0[g], f, a.arho[g]);
     }
 }
+__global__ void k_stage(StageArgs a) { stage_body(a); }
 
-// TaitEOS.loop wc/basic.py:60-65 ; TaitEOSHGCorrection.loop wc/basic.py:118-126: the pending
-// equation-of-state calls on the pool (rho clamp of the HG variant, p, cs); same arithmetic as
-// k_pack_state.  eos_tab_eval is the arithmetic on one particle's rho (clamped in place; true
-// when it was); k_eos_tab, k_pack_rec32 and the fused stage kernels all call it.
-__device__ __forceinline__ bool eos_tab_applies(const EosTab &E, const uint8_t t)
+// WCSPHTVDRK3Step stage1 / stage2 / stage3 (a.which = 1, 2, 3), real particles only;
+// its initialize is WCSPHStep's (k_stage, which = 0)
+__device__ __forceinline__ void stage_rk3_body(const StageArgs &a)
 {
-    const int a = t & 7;
-    return E.on[a] && !(E.real_only[a] && (t & PT_GHOST));
+    long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= a.pool_end) return;
+    uint8_t t = a.ptype[g];
+    if (t == PT_INVALID || (t & PT_GHOST)) return;
+    if (a.arr >= 0 && (t & 7) != a.arr) return;
+    const double dt = stage_factor(a.tc, a.f, a.which, true);
+    a.u[g] = rk3_update(a.which, a.u0[g], a.u, g, dt, a.au[g]);
+    a.v[g] = rk3_update(a.which, a.v0[g], a.v, g, dt, a.av[g]);
+    a.w[g] = rk3_update(a.which, a.w0[g], a.w, g, dt, a.aw[g]);
+    a.x[g] = rk3_update(a.which, a.x0[g], a.x, g, dt, a.ax[g]);
+    a.y[g] = rk3_update(a.which, a.y0[g], a.y, g, dt, a.ay[g]);
+    a.z[g] = rk3_update(a.which, a.z0[g], a.z, g, dt, a.az[g]);
+    a.rho[g] = rk3_update(a.which, a.rho0[g], a.rho, g, dt, a.arho[g]);
 }
-__device__ __forceinline__ bool eos_tab_eval(const EosTab &E, const int a, double &r, float &p, float &cs)
-{
-    const double rho0 = E.rho0[a];
-    const bool clamp = E.hg[a] && r < rho0;
-    if (clamp) r = rho0;
-    const double ratio = r * (1.0 / rho0);
-    const double Bc = rho0 * E.c0[a] * E.c0[a] / E.gamma[a];
-{ double rg_, rh_; tait_powers(ratio, E.gamma[a], rg_, rh_);
-    p = (float)((E.hg[a] ? 0.0 : E.p0[a]) + Bc * (rg_ - 1.0));
-    cs = (float)(E.c0[a] * rh_); }
-    return clamp;
-}
+__global__ void k_stage_rk3(StageArgs a) { stage_rk3_body(a); }
+
+// the pending equation-of-state calls on the pool (eos_tab_eval, the clamped rho written back)
 __device__ __forceinline__ void eos_tab_apply(double *__restrict__ rho, float *__restrict__ p, float *__restrict__ cs,
                                               const uint8_t t, const long long g, const EosTab &E)
 {
@@ -219,12 +253,12 @@ __device__ __forceinline__ void eos_tab_apply(double *__restrict__ rho, float *_
 //    rho of before the EOS calls below, as the reference's initialize, which runs before them]
 //   [the pool side of the last evaluation's EOS calls (k_eos_tab's arithmetic) when the pair
 //    pass left it to here: rho clamp, p, cs -- ghosts included, as k_eos_tab]
-//   stage1 / stage2 (integrator_step.py:63-91), fp64, bitwise what k_stage computes
-//     (k_stage_pack_rk3: stage1 / stage2 / stage3, :118-168, bitwise what k_stage_rk3 computes)
+//   stage1 / stage2 (integrator_step.py:63-91), fp64, wcsph_combine as k_stage
+//     (k_stage_pack_rk3: stage1 / stage2 / stage3, :118-168, rk3_combine as k_stage_rk3)
 //   the packed pair records of the NEXT evaluation at the particle's sorted slot:
-//     {A, B} = (cell-relative position of the frozen build, h, u, v, w, m)   -- k_pack_pos_light
+//     {A, B} = (cell-relative position of the frozen build, h, u, v, w, m)   -- pack_position
 //     C      = (rho, p / rho^2, cs, type) with the equation-of-state calls of the LAST
-//              evaluation applied to the record only (k_pack_state's arithmetic); the pool's
+//              evaluation applied to the record only (eos_tab_eval, state_record); the pool's
 //              rho / p / cs are written when the evaluation really issues those calls
 //   the drift of the build (max |x - x_build|^2, max (h - h_build)) into red_u32
 //   [the stepper's last stage: the adaptive-dt factors max dt_cfl, max dt_force, min h into
@@ -245,54 +279,11 @@ struct FusePackArgs {
     unsigned *red_u32;
     const float *dt_cfl, *dt_force;
     long long *red;
-    const double *tc;                // device-resident dt (tc[0]); null: StageArgs.f
     int do_init, reduce_dt, eos_any;
     EosTab E;
     int eos_pool;                    // apply EP to the pool's rho / p / cs first
     EosTab EP;
 };
-
-// WCSPHTVDRK3Step.stage1 / stage2 / stage3 (integrator_step.py:118-168) for one property, in the
-// reference's association order (rk3_combine, on the current value qc); rk3_update reads q[g]
-// for stages 2 and 3 only.  k_stage_rk3 and k_stage_pack_rk3 both go through rk3_combine, so that
-// both contract it to the same FMAs (k_stage_pack_rk3 passes rho after the pool-side EOS clamp).
-__device__ __forceinline__ double rk3_combine(const int which, const double q0, const double qc, const double dt,
-                                              const float aq)
-{
-    if (which == 1) return q0 + dt * (double)aq;
-    if (which == 2) return 0.75 * q0 + 0.25 * (qc + dt * (double)aq);
-    return (1. / 3.) * q0 + (2. / 3.) * (qc + dt * (double)aq);
-}
-__device__ __forceinline__ double rk3_update(const int which, const double q0, const double *q,
-                                             const long long g, const double dt, const float aq)
-{
-    return rk3_combine(which, q0, which == 1 ? 0.0 : q[g], dt, aq);
-}
-
-// WCSPHTVDRK3Step stage1 / stage2 / stage3 (a.which = 1, 2, 3) with dt = a.f, real particles only;
-// its initialize is WCSPHStep's (k_stage, which = 0)
-__device__ __forceinline__ void stage_rk3_body(const StageArgs &a)
-{
-    long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= a.pool_end) return;
-    uint8_t t = a.ptype[g];
-    if (t == PT_INVALID || (t & PT_GHOST)) return;
-    if (a.arr >= 0 && (t & 7) != a.arr) return;
-    const double dt = a.f;
-    a.u[g] = rk3_update(a.which, a.u0[g], a.u, g, dt, a.au[g]);
-    a.v[g] = rk3_update(a.which, a.v0[g], a.v, g, dt, a.av[g]);
-    a.w[g] = rk3_update(a.which, a.w0[g], a.w, g, dt, a.aw[g]);
-    a.x[g] = rk3_update(a.which, a.x0[g], a.x, g, dt, a.ax[g]);
-    a.y[g] = rk3_update(a.which, a.y0[g], a.y, g, dt, a.ay[g]);
-    a.z[g] = rk3_update(a.which, a.z0[g], a.z, g, dt, a.az[g]);
-    a.rho[g] = rk3_update(a.which, a.rho0[g], a.rho, g, dt, a.arho[g]);
-}
-__global__ void k_stage_rk3(StageArgs a) { stage_rk3_body(a); }
-__global__ void k_stage_rk3_devdt(StageArgs a, const double *__restrict__ tc)
-{
-    a.f = tc[0];
-    stage_rk3_body(a);
-}
 
 // The body of the fused stage kernels, the stage being WCSPHStep's or, RK3, WCSPHTVDRK3Step's.
 // s_* is the kernel's shared memory of the block reduction (one atomic per block and quantity).
@@ -310,11 +301,7 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
         if (t & PT_GHOST) {
             if (q.eos_pool) eos_tab_apply(a.rho, q.p, q.cs, t, g, q.EP);
         } else {
-            double f = a.f;
-            if (q.tc) {
-                const double dt = q.tc[0];
-                f = RK3 ? dt : (a.which == 1 ? 0.5 * dt : dt);
-            }
+            const double f = stage_factor(a.tc, a.f, a.which, RK3);
             // rho before the stage: the deferred initialize copies it as it is, the pool side of
             // the EOS calls clamps it; the stage overwrites the pool's rho, so only TVD-RK3's
             // stages 2 and 3 read the clamped value
@@ -350,13 +337,13 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
                 zn = rk3_update(a.which, z0, a.z, g, f, a.az[g]);
                 r = rk3_combine(a.which, r0, rc, f, a.arho[g]);
             } else {
-                un = u0 + f * (double)a.au[g];
-                vn = v0 + f * (double)a.av[g];
-                wn = w0 + f * (double)a.aw[g];
-                xn = x0 + f * (double)a.ax[g];
-                yn = y0 + f * (double)a.ay[g];
-                zn = z0 + f * (double)a.az[g];
-                r = r0 + f * (double)a.arho[g];
+                un = wcsph_combine(u0, f, a.au[g]);
+                vn = wcsph_combine(v0, f, a.av[g]);
+                wn = wcsph_combine(w0, f, a.aw[g]);
+                xn = wcsph_combine(x0, f, a.ax[g]);
+                yn = wcsph_combine(y0, f, a.ay[g]);
+                zn = wcsph_combine(z0, f, a.az[g]);
+                r = wcsph_combine(r0, f, a.arho[g]);
             }
             a.u[g] = un; a.v[g] = vn; a.w[g] = wn;
             a.x[g] = xn; a.y[g] = yn; a.z[g] = zn;
@@ -367,14 +354,7 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
             }
             // ---- records of the next evaluation ---------------------------------------
             const uint32_t s = q.rank[g];
-            const uint32_t key = q.key_of[g];
-            uint32_t cx, cy, cz;
-            grid_decode(q.G.zorder, (uint32_t)q.G.nc[0], (uint32_t)q.G.nc[1], key, cx, cy, cz);
-            float4 A, B, C;
-            A.x = (float)(xn - (q.G.xmin[0] + (double)cx * q.G.cell[0]));
-            A.y = (float)(yn - (q.G.xmin[1] + (double)cy * q.G.cell[1]));
-            A.z = (float)(zn - (q.G.xmin[2] + (double)cz * q.G.cell[2]));
-            A.w = (float)hg;
+            const float4 A = pack_position(q.G, q.key_of[g], xn, yn, zn, hg);
             const int ar = t & 7;
             if (q.R) {
                 // only the full sector: a lone 16-byte half would cost a read-modify-write in
@@ -384,16 +364,10 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
                 q.R[2 * (size_t)s] = R0;
                 q.R[2 * (size_t)s + 1] = R1;
             } else {
-                B.x = (float)un; B.y = (float)vn; B.z = (float)wn; B.w = (float)q.m[g];
+                const double m = q.m[g];   // read before the EOS: after it the kernel needs 64 registers, not 62
                 float pg, csg;
                 if (q.eos_any && q.E.on[ar]) {   // real particle: real_only does not matter here
-                    const double rho0 = q.E.rho0[ar];
-                    if (q.E.hg[ar] && r < rho0) r = rho0;   // the record only: the pool keeps rho
-                    const double ratio = r * (1.0 / rho0);
-                    const double Bc = rho0 * q.E.c0[ar] * q.E.c0[ar] / q.E.gamma[ar];
-{ double rg_, rh_; tait_powers(ratio, q.E.gamma[ar], rg_, rh_);
-                    pg = (float)((q.E.hg[ar] ? 0.0 : q.E.p0[ar]) + Bc * (rg_ - 1.0));
-                    csg = (float)(q.E.c0[ar] * rh_); }
+                    eos_tab_eval(q.E, ar, r, pg, csg);   // the record only: the pool keeps rho
                 } else if (eos) {
                     pg = p_eos;
                     csg = cs_eos;
@@ -401,18 +375,13 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
                     pg = q.p[g];
                     csg = q.cs[g];
                 }
-                C.x = (float)r;
-                C.y = (float)((double)pg / (r * r));
-                C.z = csg;
-                C.w = __int_as_float((int)t);
+                float4 B, C;
+                state_record(un, vn, wn, m, r, pg, csg, (int)t, B, C);
                 q.AB[2 * (size_t)s] = A;
                 q.AB[2 * (size_t)s + 1] = B;
                 q.C[s] = C;
             }
-            const float4 b0 = q.A0[s];
-            const float ex = A.x - b0.x, ey = A.y - b0.y, ez = A.z - b0.z;
-            d2 = ex * ex + ey * ey + ez * ez;
-            dh = fmaxf(A.w - b0.w, 0.f);
+            build_drift(A, q.A0[s], d2, dh);
         }
     }
 #pragma unroll
@@ -498,7 +467,7 @@ __global__ void k_pack_rec32(const double *__restrict__ u, const double *__restr
 }
 
 // the position half of AB from the 32-byte records (after k_stage_pack wrote only R):
-// the same floats k_pack_pos_light computes, for the readers of the 48-byte records
+// the floats pack_position made, for the readers of the 48-byte records
 __global__ void k_rec32_positions(const float4 *__restrict__ R, const double *__restrict__ h,
                                   const uint32_t *__restrict__ perm, long long n, float4 *__restrict__ AB)
 {
@@ -506,40 +475,6 @@ __global__ void k_rec32_positions(const float4 *__restrict__ R, const double *__
     if (s >= n) return;
     const float4 r = R[2 * s];
     AB[2 * s] = make_float4(r.x, r.y, r.z, (float)h[perm[s]]);
-}
-
-// k_dt_propose + k_dt_commit in one launch (one rank: nothing to reduce in between), and
-// the reduction slots are re-armed for the next step's fused stage kernel
-__global__ void k_dt_advance(long long *__restrict__ red, double *__restrict__ tc, double cfl, int fixed_h,
-                             double prev_factor, double new_factor, int adaptive, int advance, double t_final, double t_eps)
-{
-    if (adaptive) {
-        const double mc = o2d(red[9]), mf = o2d(red[11]);
-        const double f_cfl = mc < -1e299 ? -1.0 : mc, f_force = mf < -1e299 ? -1.0 : mf;
-        double hmin = fmin(1.0, o2d(red[12]));
-        if (!fixed_h || tc[3] < 0.0) tc[3] = hmin;
-        hmin = tc[3];
-        const double inf = __longlong_as_double(0x7ff0000000000000LL);
-        double dt_cfl = inf, dt_force = inf;
-        if (f_cfl > 0.0) dt_cfl = hmin / f_cfl;
-        if (f_force > 0.0) dt_force = sqrt(hmin / sqrt(f_force));
-        const double dt_min = fmin(dt_cfl, dt_force);
-        tc[2] = (dt_min <= 0.0 || isinf(dt_min)) ? 1e20 : cfl * dt_min;
-    }
-    red[9] = d2o(-1e300); red[11] = d2o(-1e300); red[12] = d2o(1e300);
-    const double dt_old = tc[0];
-    if (advance) tc[1] += dt_old;
-    const double t = tc[1];
-    if (fabs(t_final - t) < t_eps) return;
-    const double undamped = dt_old / prev_factor;
-    double dt = undamped;
-    if (adaptive) {
-        dt = tc[2];
-        if (dt >= 1e20) dt = undamped;
-    }
-    dt *= new_factor;
-    if (t + dt > t_final - t_eps) dt = t_final - t;
-    tc[0] = dt;
 }
 
 // _box_wrap_periodic (nnps_base.pyx:699-743): real and ghost particles alike

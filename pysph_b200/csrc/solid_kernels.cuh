@@ -352,6 +352,7 @@ struct StageSolidArgs {
     long long pool_end;
     int arr, which;
     double f;
+    const double *tc;                // device-resident dt (tc[0]); null: f
 };
 // SolidMechStep integrator_step.py:173-252 (real particles)
 __device__ __forceinline__ void stage_solid_body(const StageSolidArgs &a)
@@ -369,7 +370,7 @@ __device__ __forceinline__ void stage_solid_body(const StageSolidArgs &a)
         for (int k = 0; k < 6; k++) a.s0[k][g] = a.s[k][g];
         return;
     }
-    const double f = a.f;
+    const double f = stage_factor(a.tc, a.f, a.which, false);
     a.u[g] = a.u0[g] + f * (double)a.au[g];
     a.v[g] = a.v0[g] + f * (double)a.av[g];
     a.w[g] = a.w0[g] + f * (double)a.aw[g];
@@ -381,12 +382,6 @@ __device__ __forceinline__ void stage_solid_body(const StageSolidArgs &a)
     for (int k = 0; k < 6; k++) a.s[k][g] = a.s0[k][g] + f * (double)a.as[k][g];
 }
 __global__ void k_stage_solid(StageSolidArgs a) { stage_solid_body(a); }
-__global__ void k_stage_solid_devdt(StageSolidArgs a, const double *__restrict__ tc)
-{
-    const double dt = tc[0];
-    a.f = a.which == 1 ? 0.5 * dt : dt;
-    stage_solid_body(a);
-}
 
 // refresh the packed positions in the FROZEN sorted order / cell frames of the last
 // build and measure how far particles moved (and h grew) since then.
@@ -402,20 +397,10 @@ __global__ void k_pack_pos_light(const double *__restrict__ x, const double *__r
     float d2 = 0.f, dh = 0.f;
     if (s < n) {
         const uint32_t g = perm[s];
-        uint32_t key = skey[s];
-        uint32_t cx, cy, cz;
-        grid_decode(G.zorder, (uint32_t)G.nc[0], (uint32_t)G.nc[1], key, cx, cy, cz);
-        float4 a;
-        a.x = (float)(x[g] - (G.xmin[0] + (double)cx * G.cell[0]));
-        a.y = (float)(y[g] - (G.xmin[1] + (double)cy * G.cell[1]));
-        a.z = (float)(z[g] - (G.xmin[2] + (double)cz * G.cell[2]));
-        a.w = (float)h[g];
+        const float4 a = pack_position(G, skey[s], x[g], y[g], z[g], h[g]);
         A[s] = a;
         AB[2 * s] = a;
-        const float4 b = A0[s];
-        const float dx = a.x - b.x, dy = a.y - b.y, dz = a.z - b.z;
-        d2 = dx * dx + dy * dy + dz * dz;
-        dh = fmaxf(a.w - b.w, 0.f);
+        build_drift(a, A0[s], d2, dh);
     }
     for (int o = 16; o > 0; o >>= 1) {
         d2 = fmaxf(d2, __shfl_xor_sync(0xffffffffu, d2, o));

@@ -394,6 +394,7 @@ struct StageTvfArgs {
     long long pool_end;
     int arr, which;
     double f;
+    const double *tc;                // device-resident dt (tc[0]); null: f
     // EDACStep (wc/edac.py:82-133, the scheme without transport velocity): positions move with
     // the XSPH-corrected velocity ax ay az, there is no uhat
     int ext;
@@ -413,7 +414,7 @@ __device__ __forceinline__ void stage_tvf_body(const StageTvfArgs &a)
         a.pf0[g] = a.pf[g];
         return;
     }
-    const double f = a.f;
+    const double f = stage_factor(a.tc, a.f, a.which, false);
     const double u = a.u0[g] + f * (double)a.au[g];
     const double v = a.v0[g] + f * (double)a.av[g];
     const double w = a.w0[g] + f * (double)a.aw[g];
@@ -434,9 +435,3 @@ __device__ __forceinline__ void stage_tvf_body(const StageTvfArgs &a)
     a.pf[g] = a.pf0[g] + f * (double)a.ap[g];
 }
 __global__ void k_stage_tvf(StageTvfArgs a) { stage_tvf_body(a); }
-__global__ void k_stage_tvf_devdt(StageTvfArgs a, const double *__restrict__ tc)
-{
-    const double dt = tc[0];
-    a.f = a.which == 1 ? 0.5 * dt : dt;
-    stage_tvf_body(a);
-}
