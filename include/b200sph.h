@@ -334,6 +334,26 @@ int b200sph_generic_load(b200sph_ctx *ctx, const void *image, int64_t size);
 int b200sph_generic_launch(b200sph_ctx *ctx, int module, const char *kernel, int dest_arr, int phase,
                            unsigned src_mask, int real_only, double t, double dt, int writes);
 
+/* ---- density re-initialisation: DensityCorrection (pysph/solver/tools.py:97-205) ----------
+ * One Group([Filter(a, [a])], real=False) per array a of array_mask, Filter one of ShepardFilter,
+ * MLSFirstOrder2D, MLSFirstOrder3D (pysph/sph/wc/density_correction.py): rhotmp = rho, then rho
+ * from the rhotmp of the array's own particles over the persistent neighbour lists.  `kernel`
+ * (B200SPH_KERNEL_*) is the filter's smoothing kernel, which may differ from the evaluation's; its
+ * radius scale must not exceed that of b200sph_set_kernel.  rhotmp_prop: a user property
+ * (b200sph_user_property).  real_only: the Group's real=True (only real destinations).
+ * p and cs are left alone; the next evaluation's equation of state and records see the new
+ * rho.  Refused: periodic or mirror domains, the slab decomposition, lists that cannot index
+ * the particles, MLS2D with dim != 2 and MLS3D with dim != 3.
+ * A new symbol only: no structure and no b200sph_stats counter changed, so
+ * B200SPH_ABI_VERSION stays 5. */
+enum {
+    B200SPH_DFILTER_SHEPARD = 0,
+    B200SPH_DFILTER_MLS2D = 1,
+    B200SPH_DFILTER_MLS3D = 2
+};
+int b200sph_density_filter(b200sph_ctx *ctx, uint32_t array_mask, int mode, int kernel, int rhotmp_prop,
+                           int real_only);
+
 /* The two Groups of EDACScheme._get_internal_flow_equations (wc/edac.py:776-880) in
  * the generated AccelerationEval.compute (acceleration_eval_cython.mako:10-154): group 1 computes
  * V = sum W, rho = m V (transport_velocity.py:24-58) and the neighbour-average

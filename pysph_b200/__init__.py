@@ -15,6 +15,7 @@ DeviceHelper (``pa.gpu``)   :class:`B200DeviceHelper` / :class:`B200Backend`
 Equation / Group            :mod:`pysph_b200.equations`
 WCSPHScheme.get_equations   :class:`pysph_b200.scheme.WCSPHScheme`
 Solver step loop            :class:`B200Solver`
+solver tools                :class:`DensityCorrection`
 ParallelManager             :class:`pysph_b200.parallel.SlabParallelManager`
 ==========================  ==================================================
 
@@ -29,7 +30,8 @@ from .kernels import CubicSpline, WendlandQuintic, QuinticSpline, Gaussian
 from .equations import (Equation, Group, SummationDensity, ContinuityEquation, LaminarViscosity,
                         MonaghanArtificialViscosity, XSPHCorrection, TaitEOS,
                         TaitEOSHGCorrection, MomentumEquation,
-                        UpdateSmoothingLengthFerrari)
+                        UpdateSmoothingLengthFerrari, ShepardFilter, MLSFirstOrder2D,
+                        MLSFirstOrder3D)
 from .scheme import WCSPHScheme
 from .backend import B200Backend, B200DeviceHelper
 from .domain import DomainManager
@@ -38,6 +40,7 @@ from .acceleration_eval import B200AccelerationEval
 from .integrator import (B200Integrator, PECIntegrator, EPECIntegrator,
                          TVDRK3Integrator, WCSPHStep, WCSPHTVDRK3Step)
 from .solver import B200Solver
+from .tools import Tool, DensityCorrection
 from .edac import EDACScheme, EDACTVFStep, EDACStep
 from .output import dump, load
 from .solid_mech import ElasticSolidsScheme, SolidMechStep

@@ -13,6 +13,14 @@ from .kernels import kernel_id
 from .program import build_program, index_value, _converged
 
 
+def _has_op(ops, kind):
+    """an op of this kind anywhere in the (nested) op list"""
+    for op in ops:
+        if op[0] == kind or any(isinstance(x, list) and _has_op(x, kind) for x in op[1:]):
+            return True
+    return False
+
+
 class B200AccelerationEval(object):
     def __init__(self, particle_arrays, equations, kernel, backend=None,
                  mode='serial', device=0):
@@ -46,6 +54,10 @@ class B200AccelerationEval(object):
         # properties the generated kernels use beyond the pool's own
         for name in self._generic_props.user:
             self.backend.add_user_property(name)
+        # the density filters' rhotmp (a user property: push / pull / resize carry it)
+        self._rhotmp = self.backend.add_user_property('rhotmp') \
+            if _has_op(self.ops, 'dfilter') else None
+        self._kid = kernel_id(kernel)
         self._range = None
         self.nnps = None
         self.count_pairs = False
@@ -129,6 +141,9 @@ class B200AccelerationEval(object):
                     self._pairs += cnt.value
                 else:
                     ctx.call('b200sph_solid_pass', C.byref(op[1]), None)
+            elif kind == 'dfilter':
+                _, mode, mask, real_only = op
+                ctx.call('b200sph_density_filter', mask, mode, self._kid, self._rhotmp, real_only)
             elif kind == 'update_nnps':
                 # mako:139-145: nnps.update_domain(); nnps.update()
                 ctx.call('b200sph_update_domain')

@@ -395,6 +395,9 @@ struct b200sph_ctx {
     // generic-equation fallback: user properties (fp64, pool-wide) and run-time compiled modules
     double *user_f64[B200SPH_MAX_USER] = {nullptr};
     std::vector<void *> gen_modules;             // CUmodule (or, emulated, a dlopen handle)
+    // density_filter: its records, [2 n_sorted] (allocated on first use)
+    float4 *dfilter_F = nullptr;
+    size_t dfilter_cap = 0;
     // Group(start_idx, stop_idx): one-shot destination ranges of the next pair pass
     int64_t dst_lo[B200SPH_MAX_ARRAYS] = {0}, dst_hi[B200SPH_MAX_ARRAYS] = {0};
     bool dst_ranged = false;
@@ -654,6 +657,7 @@ __device__ __forceinline__ void rec32_make(const float4 A, const double u, const
 #include "tvf_kernels.cuh"
 #include "solid_kernels.cuh"
 #include "halo_kernels.cuh"
+#include "density_filter.cuh"
 
 // --------------------------------------------------------------------------
 // host side
@@ -924,16 +928,20 @@ PhaseTimer::~PhaseTimer()
 // The (kernel, dim) pairs the templated pair-walking kernels are instantiated for: every kernel
 // in 1-3 dimensions except WendlandQuintic in 1-D (b200sph_set_kernel refuses it).  `launch`
 // gets them as std::integral_constant<int, K> and std::integral_constant<int, DIM>.
-template <class F> static int with_kernel_dim(b200sph_ctx *ctx, const char *who, F &&launch)
+template <class F> static int with_kernel_dim(b200sph_ctx *ctx, int kernel, int dim, const char *who, F &&launch)
 {
     using std::integral_constant;
-    switch (ctx->kernel * 4 + ctx->dim) {
+    switch (kernel * 4 + dim) {
 #define KD(K, D) \
     case K * 4 + D: return launch(integral_constant<int, K>(), integral_constant<int, D>());
         KD(0, 1) KD(0, 2) KD(0, 3) KD(1, 2) KD(1, 3) KD(2, 1) KD(2, 2) KD(2, 3) KD(3, 1) KD(3, 2) KD(3, 3)
 #undef KD
     default: return set_err(ctx, "%s: unsupported kernel/dim combination", who);
     }
+}
+template <class F> static int with_kernel_dim(b200sph_ctx *ctx, const char *who, F &&launch)
+{
+    return with_kernel_dim(ctx, ctx->kernel, ctx->dim, who, launch);
 }
 
 // with the elastic-dynamics arrays allocated the deviatoric stress travels too: a ghost is a
@@ -1018,6 +1026,10 @@ static double kernel_fac(int kernel, int dim)
     default: return std::pow(1.0 / std::sqrt(pi), dim);                                // kernels.py:852-858
     }
 }
+static double kernel_radius_scale(int kernel)
+{
+    return (kernel == B200SPH_KERNEL_QUINTIC_SPLINE || kernel == B200SPH_KERNEL_GAUSSIAN) ? 3.0 : 2.0;
+}
 static double kernel_deltap(int kernel)
 {
     switch (kernel) {
@@ -1095,7 +1107,7 @@ int b200sph_destroy(b200sph_ctx *ctx)
     for (int k = 0; k < B200SPH_MAX_USER; k++) cudaFree(ctx->user_f64[k]);
     generic_unload_all(ctx);
     for (int k = 0; k < N_F32X; k++) cudaFree(ctx->f32x[k]);
-    cudaFree(ctx->Dv); cudaFree(ctx->PT);
+    cudaFree(ctx->Dv); cudaFree(ctx->PT); cudaFree(ctx->dfilter_F);
     for (auto &sg : ctx->mirror_segs) cudaFree(sg.idx);
     for (int k = 0; k < 12; k++) cudaFree(ctx->f64s[k]);
     for (int k = 0; k < 21; k++) cudaFree(ctx->f32s[k]);
@@ -1473,7 +1485,7 @@ int b200sph_set_kernel(b200sph_ctx *ctx, int kernel, int dim)
         return set_err(ctx, "WendlandQuintic: Dim 1 not supported");  // kernels.py:289-290
     ctx->kernel = kernel;
     ctx->dim = dim;
-    ctx->radius_scale = (kernel == B200SPH_KERNEL_QUINTIC_SPLINE || kernel == B200SPH_KERNEL_GAUSSIAN) ? 3.0 : 2.0;
+    ctx->radius_scale = kernel_radius_scale(kernel);
     h_changed(ctx);   // (the cell size is radius_scale hmax)
     build_invalid(ctx);
     return 0;
@@ -2365,6 +2377,77 @@ int b200sph_generic_launch(b200sph_ctx *ctx, int module, const char *kernel, int
     // what was derived from the properties the bodies stored to is stale
     if (writes & 1) h_changed(ctx);
     if (writes & 2) state_changed(ctx), m_changed(ctx), ctx->spec_records = false;
+    return 0;
+}
+
+// DensityCorrection's filter (density_filter.cuh).  Like generic_launch, a list consumer that
+// writes a pool property between evaluations: the deferred initialize has copied the rho it
+// overwrites (ensure_pool), the pending EOS calls are in the pool, and afterwards everything
+// made from rho -- the packed records, the EOS speculatively applied to them -- is stale.
+int b200sph_density_filter(b200sph_ctx *ctx, uint32_t array_mask, int mode, int kernel, int rhotmp_prop, int real_only)
+{
+    if (int rcc = require_confirmed(ctx, "density_filter")) return rcc;
+    CU(cudaSetDevice(ctx->device));
+    int rc = ensure_pool(ctx);
+    if (rc) return rc;
+    if (mode < B200SPH_DFILTER_SHEPARD || mode > B200SPH_DFILTER_MLS3D) return set_err(ctx, "density_filter: unknown mode %d", mode);
+    if (kernel < 0 || kernel > 3) return set_err(ctx, "density_filter: unknown kernel id %d", kernel);
+    if (kernel == B200SPH_KERNEL_WENDLAND_QUINTIC && ctx->dim == 1) return set_err(ctx, "WendlandQuintic: Dim 1 not supported");
+    if (mode == B200SPH_DFILTER_MLS2D && ctx->dim != 2) return set_err(ctx, "density_filter: MLSFirstOrder2D needs dim = 2 (dim is %d)", ctx->dim);
+    if (mode == B200SPH_DFILTER_MLS3D && ctx->dim != 3) return set_err(ctx, "density_filter: MLSFirstOrder3D needs dim = 3 (dim is %d)", ctx->dim);
+    if (array_mask == 0 || array_mask >= (1u << ctx->narr)) return set_err(ctx, "density_filter: bad array mask 0x%x", array_mask);
+    if (!is_user_prop(rhotmp_prop) || !ctx->user_f64[rhotmp_prop - B200SPH_USER0])
+        return set_err(ctx, "density_filter: rhotmp (property %d) is not a user property (b200sph_user_property)", rhotmp_prop);
+    if (ctx->peer_box || ctx->comm_pending) return set_err(ctx, "density_filter runs on one GPU (no slab decomposition)");
+    if (ctx->periodic[0] || ctx->periodic[1] || ctx->periodic[2] || mirror_any(ctx))
+        return set_err(ctx, "density_filter: periodic and mirror domains are not supported");
+    if (kernel_radius_scale(kernel) > ctx->radius_scale)
+        return set_err(ctx, "density_filter: the filter kernel's radius scale (%g) exceeds the evaluation kernel's (%g), "
+                            "which the neighbour lists are built for", kernel_radius_scale(kernel), ctx->radius_scale);
+    if (!ctx->grid_valid) return set_err(ctx, "density_filter: the NNPS is stale (particles were pushed/resized); call nnps_update first");
+    if ((rc = eos_flush(ctx)) || (rc = ab_positions(ctx))) return rc;
+    if (ctx->n_sorted > 0) {
+        // every filtered array is its own (only) source; the lists keep the union of what was asked
+        unsigned long long want[B200SPH_MAX_ARRAYS] = {0};
+        for (int a = 0; a < ctx->narr; a++)
+            if ((array_mask >> a) & 1u) want[a] |= 0xFFull << (8 * a);
+        if ((rc = prepare_lists(ctx, want, "density_filter: the neighbour lists cannot index the particles"))) return rc;
+        if ((size_t)ctx->n_sorted > ctx->dfilter_cap) {
+            if (ctx->dfilter_F) CU(cudaFree(ctx->dfilter_F));
+            ctx->dfilter_F = nullptr;
+            CU(cudaMalloc((void **)&ctx->dfilter_F, 2 * sizeof(float4) * (size_t)ctx->n_sorted));
+            ctx->dfilter_cap = (size_t)ctx->n_sorted;
+        }
+        PhaseTimer pt(ctx, 1);
+        DensityFilterArgs fa;
+        memset(&fa, 0, sizeof(fa));
+        fa.AB = ctx->AB; fa.F = ctx->dfilter_F;
+        fa.perm = ctx->perm; fa.cnt = ctx->cnt; fa.lst = ctx->lst; fa.stype = ctx->stype;
+        fa.m = ctx->f64[B200SPH_M]; fa.rho = ctx->f64[B200SPH_RHO]; fa.rhotmp = ctx->user_f64[rhotmp_prop - B200SPH_USER0];
+        fa.n = ctx->n_sorted; fa.capg = ctx->capg;
+        fa.cellx = (float)ctx->G.cell[0]; fa.celly = (float)ctx->G.cell[1]; fa.cellz = (float)ctx->G.cell[2];
+        const double kr = kernel_radius_scale(kernel);
+        fa.k2 = (float)(kr * kr);
+        fa.kfac = (float)kernel_fac(kernel, ctx->dim);
+        fa.mask = array_mask;
+        fa.real_only = real_only;
+        k_dfilter_pack<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(fa);
+        LAUNCH_CHECK();
+        const unsigned nb = (unsigned)cdiv(ctx->n_sorted, DFILTER_NT);
+        rc = with_kernel_dim(ctx, kernel, ctx->dim, "density_filter", [&](auto kc, auto dc) {
+            constexpr int K = decltype(kc)::value, D = decltype(dc)::value;
+            if (mode == B200SPH_DFILTER_SHEPARD) k_density_filter<K, D, B200SPH_DFILTER_SHEPARD><<<nb, DFILTER_NT, 0, ctx->stream>>>(fa);
+            else if constexpr (D == 2) k_density_filter<K, 2, B200SPH_DFILTER_MLS2D><<<nb, DFILTER_NT, 0, ctx->stream>>>(fa);
+            else if constexpr (D == 3) k_density_filter<K, 3, B200SPH_DFILTER_MLS3D><<<nb, DFILTER_NT, 0, ctx->stream>>>(fa);
+            LAUNCH_CHECK();
+            return 0;
+        });
+        if (rc) return rc;
+        ctx->stats.kernel_launches += 2;
+    }
+    // rho changed: the next evaluation packs its records (and applies its EOS) from it
+    state_changed(ctx);
+    ctx->spec_records = false;
     return 0;
 }
 

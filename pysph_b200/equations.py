@@ -141,3 +141,18 @@ class UpdateSmoothingLengthFerrari(Equation):
         self.dim1 = 1. / dim
         self.hdx = hdx
         super(UpdateSmoothingLengthFerrari, self).__init__(dest, sources)
+
+
+class ShepardFilter(Equation):
+    """Zeroth-order density re-initialisation, wc/density_correction.py:7-46:
+    rho_a = sum_b m_b W_ab / sum_b (m_b / rhotmp_b) W_ab"""
+
+
+class MLSFirstOrder2D(Equation):
+    """First-order moving-least-squares density re-initialisation in 2-D,
+    wc/density_correction.py:49-140"""
+
+
+class MLSFirstOrder3D(Equation):
+    """First-order moving-least-squares density re-initialisation in 3-D,
+    wc/density_correction.py:143-205"""

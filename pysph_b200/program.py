@@ -9,6 +9,7 @@ recognises each equation by *class name* and maps every Group onto
     ('ferrari', arr, hdx, dim, real_only)                 no-source loop
     ('pair', PairProgram)                                  fused pair kernel
     ('update_nnps',)                                       Group(update_nnps=True)
+    ('dfilter', mode, array_mask, real_only)              density re-initialisation
 
 Anything the CUDA library has no kernel for raises NotImplementedError here,
 i.e. at setup time, never silently at run time.
@@ -54,10 +55,19 @@ SOLID_GROUP2 = ('ContinuityEquation', 'MomentumEquationWithStress',
                 'XSPHCorrection')
 
 
+# density re-initialisation (wc/density_correction.py): a Group of one of them -> one
+# ('dfilter', ...) op (k_density_filter)
+DFILTER_EQUATIONS = {
+    'ShepardFilter': _lib.DFILTER_SHEPARD,
+    'MLSFirstOrder2D': _lib.DFILTER_MLS2D,
+    'MLSFirstOrder3D': _lib.DFILTER_MLS3D,
+}
+
 # every equation that has a hand-written kernel; a Group made ONLY of others takes the
 # generic-equation fallback (pysph_b200/codegen.py)
 KNOWN_EQUATIONS = set(PAIR_EQUATIONS) | set(NO_SOURCE_EQUATIONS) | set(TVF_GROUP1) | \
-    set(TVF_WALL) | set(TVF_WALL_OPTIONAL) | set(TVF_GROUP2) | set(SOLID_GROUP1) | set(SOLID_GROUP2)
+    set(TVF_WALL) | set(TVF_WALL_OPTIONAL) | set(TVF_GROUP2) | set(SOLID_GROUP1) | \
+    set(SOLID_GROUP2) | set(DFILTER_EQUATIONS)
 import itertools
 _generic_uid = itertools.count()
 
@@ -499,10 +509,36 @@ def _leaf_group(g, index, arrays, particle_arrays):
     return ops
 
 
+def _build_dfilter(g, index, ranged):
+    """A Group of density filters of one kind, each with its destination as its only source
+    (what DensityCorrection builds, tools.py:133-188) -> ('dfilter', mode, array_mask, real_only)."""
+    names = sorted(set(_eq_name(e) for e in g.equations))
+    if len(names) != 1 or names[0] not in DFILTER_EQUATIONS:
+        raise NotImplementedError(
+            'B200 backend: a density filter (%s) cannot share a Group with other equations or '
+            'another filter kind; got %s' % (', '.join(sorted(DFILTER_EQUATIONS)), names))
+    _no_range(g, ranged, 'density-filter')
+    mask = 0
+    for eq in g.equations:
+        if eq.dest not in index:
+            raise ValueError('equation %s: unknown destination array %r' % (names[0], eq.dest))
+        if list(eq.sources or []) != [eq.dest]:
+            # the reference runs loop_all once per source, each starting from rho = 0: the last
+            # source would win
+            raise NotImplementedError(
+                'B200 backend: %s(dest=%r, sources=%r): the filter takes its destination as '
+                'its only source' % (names[0], eq.dest, eq.sources))
+        mask |= 1 << index[eq.dest]
+    real_only = 1 if getattr(g, 'real', True) else 0
+    return [('dfilter', DFILTER_EQUATIONS[names[0]], mask, real_only)]
+
+
 def _leaf_body(g, index, arrays, particle_arrays):
     ops = []
     start, stop = getattr(g, 'start_idx', 0), getattr(g, 'stop_idx', None)
     ranged = (stop is not None) or (start not in (0, None))
+    if any(_eq_name(e) in DFILTER_EQUATIONS for e in g.equations):
+        return _build_dfilter(g, index, ranged)
     from . import codegen
     # a Group with at least one equation the library has no kernel for, all of whose equations
     # carry Python bodies (the reference's own objects always do; this package's descriptors of

@@ -48,6 +48,7 @@ class B200Solver(object):
         self.pre_step_callbacks = []
         self.post_step_callbacks = []
         self.post_stage_callbacks = []
+        self.tools = []
         self.max_steps = 1 << 31
         self.pfreq = 100
         self.disable_output = True   # nothing is written unless a directory is set
@@ -87,6 +88,18 @@ class B200Solver(object):
         then needs t and dt at every stage: the time step stays on the host."""
         self.post_stage_callbacks.append(callback)
         self.integrator.set_post_stage_callback(self._post_stage_callback)
+
+    def add_tool(self, tool):
+        """Application.add_tool (application.py:1358-1369, :1470-1475): register the
+        pre_step / post_stage / post_step methods the tool overloads."""
+        from .tools import is_overloaded_method
+        if is_overloaded_method(tool, 'pre_step'):
+            self.add_pre_step_callback(tool.pre_step)
+        if is_overloaded_method(tool, 'post_stage'):
+            self.add_post_stage_callback(tool.post_stage)
+        if is_overloaded_method(tool, 'post_step'):
+            self.add_post_step_callback(tool.post_step)
+        self.tools.append(tool)
 
     def _post_stage_callback(self, time, dt, stage):     # solver.py:781-785
         for callback in self.post_stage_callbacks:
