@@ -598,24 +598,9 @@ __device__ __forceinline__ float frsqrt(float x)
     return r;
 }
 
-// A float4 table in shared memory read through an opaque 32-bit shared address: the
-// compiler otherwise re-derives the CTA's shared window base (three uniform instructions)
-// at every use inside the pair loops.  (The host emulation of the tests supplies its own.)
+// nanosecond clock shared by every SM (bounds the spin waits of the peer protocol); the
+// host emulation of the tests supplies its own
 #ifndef B200SPH_HOST_EMULATION
-typedef uint32_t smem_tab_t;
-__device__ __forceinline__ smem_tab_t smem_tab(const float4 *table)
-{
-    uint32_t a = (uint32_t)__cvta_generic_to_shared(table);
-    asm volatile("" : "+r"(a));
-    return a;
-}
-__device__ __forceinline__ float4 lds_T(const smem_tab_t t, const uint32_t index)
-{
-    float4 v;
-    asm("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(t + (index << 4)));
-    return v;
-}
-// nanosecond clock shared by every SM (bounds the spin waits of the peer protocol)
 __device__ __forceinline__ unsigned long long peer_now_ns()
 {
     unsigned long long t;

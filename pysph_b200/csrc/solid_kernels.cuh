@@ -382,82 +382,3 @@ __device__ __forceinline__ void stage_solid_body(const StageSolidArgs &a)
     for (int k = 0; k < 6; k++) a.s[k][g] = a.s0[k][g] + f * (double)a.as[k][g];
 }
 __global__ void k_stage_solid(StageSolidArgs a) { stage_solid_body(a); }
-
-// refresh the packed positions in the FROZEN sorted order / cell frames of the last
-// build and measure how far particles moved (and h grew) since then.
-// red_u32[0] = max |dx|^2 (float bits), red_u32[1] = max (h - h_build) (float bits, >= 0)
-__global__ void k_pack_pos_light(const double *__restrict__ x, const double *__restrict__ y,
-                                 const double *__restrict__ z, const double *__restrict__ h,
-                                 const uint32_t *__restrict__ perm, const uint32_t *__restrict__ skey,
-                                 long long n, GridDev G, const float4 *__restrict__ A0,
-                                 float4 *__restrict__ A, float4 *__restrict__ AB,
-                                 unsigned *__restrict__ red_u32)
-{
-    long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    float d2 = 0.f, dh = 0.f;
-    if (s < n) {
-        const uint32_t g = perm[s];
-        const float4 a = pack_position(G, skey[s], x[g], y[g], z[g], h[g]);
-        A[s] = a;
-        AB[2 * s] = a;
-        build_drift(a, A0[s], d2, dh);
-    }
-    for (int o = 16; o > 0; o >>= 1) {
-        d2 = fmaxf(d2, __shfl_xor_sync(0xffffffffu, d2, o));
-        dh = fmaxf(dh, __shfl_xor_sync(0xffffffffu, dh, o));
-    }
-    if ((threadIdx.x & 31) == 0) {
-        if (d2 > 0.f) atomicMax(&red_u32[0], __float_as_uint(d2));
-        if (dh > 0.f) atomicMax(&red_u32[1], __float_as_uint(dh));
-    }
-}
-
-
-// neighbour query for one destination particle with the pair kernel's accept test
-// (cell by cell; periodic axes wrap).  One warp.
-__global__ void k_neighbors(const float4 *__restrict__ A /* {A,B} interleaved: A of particle s at [2 s] */, const float4 *__restrict__ C,
-                            const uint32_t *__restrict__ cell_start, const uint32_t *__restrict__ skey,
-                            const uint32_t *__restrict__ perm, long long s, int src_arr,
-                            long long src_off, GridDev G, float k2,
-                            uint32_t *__restrict__ out, long long cap, unsigned long long *count)
-{
-    const int lane = threadIdx.x;
-    const int ncx = G.nc[0], ncy = G.nc[1], ncz = G.nc[2];
-    const float4 Ai = A[2 * (size_t)s];
-    uint32_t kq = skey[s];
-    uint32_t ucx, ucy, ucz;
-    grid_decode(G.zorder, (uint32_t)ncx, (uint32_t)ncy, kq, ucx, ucy, ucz);
-    const int cx = (int)ucx, cy = (int)ucy, cz = (int)ucz;
-    const float hi2 = k2 * Ai.w * Ai.w;
-    unsigned long long n = 0;
-    for (int r = 0; r < 27; r++) {
-        const int dx = (r % 3) - 1, dy = ((r / 3) % 3) - 1, dz = (r / 9) - 1;
-        int xx = cx + dx, yy = cy + dy, zz = cz + dz;
-        if (G.periodic[0]) xx = (xx + ncx) % ncx;
-        if (G.periodic[1]) yy = (yy + ncy) % ncy;
-        if (G.periodic[2]) zz = (zz + ncz) % ncz;
-        if (xx < 0 || xx >= ncx || yy < 0 || yy >= ncy || zz < 0 || zz >= ncz) continue;
-        const uint32_t c = (uint32_t)xx + (uint32_t)ncx * grid_row(G.zorder, (uint32_t)ncy, (uint32_t)yy, (uint32_t)zz);
-        const uint32_t rs = cell_start[c], re = cell_start[c + 1];
-        for (uint32_t t0 = rs; t0 < re; t0 += 32) {
-            const uint32_t t = t0 + lane;
-            bool ok = false;
-            if (t < re) {
-                const float4 Aj = A[2 * (size_t)t];
-                const float xij = Ai.x - (float)dx * (float)G.cell[0] - Aj.x;
-                const float yij = Ai.y - (float)dy * (float)G.cell[1] - Aj.y;
-                const float zij = Ai.z - (float)dz * (float)G.cell[2] - Aj.z;
-                const float r2 = xij * xij + yij * yij + zij * zij;
-                ok = ((r2 < hi2) || (r2 < k2 * Aj.w * Aj.w)) &&
-                     ((__float_as_int(C[t].w) & 7) == src_arr);
-            }
-            const unsigned m = __ballot_sync(0xffffffffu, ok);
-            if (ok) {
-                const unsigned long long pos = n + __popc(m & ((1u << lane) - 1u));
-                if ((long long)pos < cap) out[pos] = (uint32_t)((long long)perm[t] - src_off);
-            }
-            n += __popc(m);
-        }
-    }
-    if (lane == 0) *count = n;
-}

@@ -115,12 +115,10 @@ static inline float frcp(float x) { return 1.0f / x; }
 static inline float frsqrt(float x) { return 1.0f / sqrtf(x); }
 static inline void ld_256(const float4 *p, float4 &b, float4 &c) { b = p[0]; c = p[1]; }
 
-// smem_tab_t / smem_tab / lds_T: inline PTX in the CUDA build
+// b200sph.cu replaces peer_now_ns (inline PTX, defined below) and the driver-API module
+// loading under this macro
 #define B200SPH_HOST_EMULATION 1
-typedef const float4 *smem_tab_t;
 template <class T> static inline T __ldg(const T *p) { return *p; }
-static inline smem_tab_t smem_tab(const float4 *table) { return table; }
-static inline float4 lds_T(smem_tab_t t, uint32_t index) { return t[index]; }
 using std::isinf;
 using std::max;
 using std::min;

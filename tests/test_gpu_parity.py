@@ -115,6 +115,8 @@ def test_wcsph_evaluation_vs_reference_bodies(gpu_device, idx):
         B = case['params']['rho0'] * case['params']['c0'] ** 2 / case['params']['gamma']
         assert np.allclose(pa.p, ref['p'], rtol=2e-5 if sd else 1e-6,
                            atol=(2e-5 * B) if sd else 1e-3)
+        # (with summation density that atol is wider than TOL_EVAL * max|p|)
+        assert rel_err(pa.p, ref['p']) <= TOL_EVAL, (pa.name, 'p', rel_err(pa.p, ref['p']))
         assert np.allclose(pa.cs, ref['cs'], rtol=2e-6)
         assert np.allclose(pa.rho, ref['rho'], rtol=2e-6 if case['params'][
             'summation_density'] else 1e-15)
@@ -662,11 +664,26 @@ def test_zorder_rows_give_the_same_neighbours_and_fields(gpu_device, monkeypatch
     """B200SPH_ZORDER=1 orders the cell rows along the Z-curve of (cy, cz) (north_star's
     "Z-curve cell list"; z_order_nnps.pyx:252-355 sorts by the 3-D Morton key): only the
     order in which neighbours are visited changes -- identical pair counts, neighbour sets
-    and (to fp32 summation order) fields, through list rebuilds."""
+    and (to fp32 summation order) fields, through list rebuilds.  In either order one
+    evaluation of a coarser perturbed dam break matches the oracle: pair count, every
+    acceleration-like field, p and cs."""
     import pysph_b200 as pb
+    opas, oparams = _perturbed_dam_break(dx=0.09, seed=5)
+    o = orc.WCSPHOracleSolver(opas, oparams, 'CubicSpline')
+    want_pairs = o.evaluate()
     out = {}
     for z in ('0', '1'):
         monkeypatch.setenv('B200SPH_ZORDER', z)
+        pas, params = _perturbed_dam_break(dx=0.09, seed=5)
+        s = make_solver(pas, scheme_params(params), 'CubicSpline')
+        s.a_eval.count_pairs = True
+        s.a_eval.compute(0.0, 0.0)
+        s.pull()
+        assert s.a_eval.last_pairs == want_pairs, z
+        for pa, oa in zip(pas, opas):
+            for k in ACC_FIELDS + ['p', 'cs']:
+                err = rel_err(pa.properties[k], oa.properties[k])
+                assert err <= TOL_EVAL, (z, pa.name, k, err)
         pas, params = _perturbed_dam_break(vscale=3.0)
         s = make_solver(pas, scheme_params(params), 'CubicSpline')
         s.a_eval.count_pairs = True

@@ -7,7 +7,7 @@ pysph/tools/tests/test_sph_evaluator.py:36-52."""
 import numpy as np
 import pytest
 
-from helpers import rel_err
+from helpers import ACC_FIELDS, rel_err
 from oracle import oracle as orc
 
 pytestmark = pytest.mark.gpu
@@ -133,22 +133,30 @@ def _periodic_case(dim, n, seed=3, tensile=True):
     return pa, params
 
 
-@pytest.mark.parametrize('dim,n,pattern,tensile', [
-    pytest.param(2, 24, (1, 1, 0), True, id='2-24-pattern0'),
-    pytest.param(3, 10, (1, 1, 1), True, id='3-10-pattern1'),
-    pytest.param(3, 10, (1, 0, 1), True, id='3-10-pattern2'),
-    pytest.param(2, 24, (0, 1, 0), True, id='2-24-pattern3'),
-    pytest.param(2, 24, (1, 1, 0), False, id='2-24-pattern0-no_tensile'),
-    pytest.param(3, 10, (1, 0, 1), False, id='3-10-pattern2-no_tensile')])
-def test_periodic_wcsph_steps_vs_oracle(gpu_device, dim, n, pattern, tensile):
-    periodic_wcsph_steps_vs_oracle(gpu_device, dim, n, pattern, tensile)
+@pytest.mark.parametrize('dim,n,pattern,tensile,zorder', [
+    pytest.param(2, 24, (1, 1, 0), True, False, id='2-24-pattern0'),
+    pytest.param(3, 10, (1, 1, 1), True, False, id='3-10-pattern1'),
+    pytest.param(3, 10, (1, 0, 1), True, False, id='3-10-pattern2'),
+    pytest.param(2, 24, (0, 1, 0), True, False, id='2-24-pattern3'),
+    pytest.param(2, 24, (1, 1, 0), False, False, id='2-24-pattern0-no_tensile'),
+    pytest.param(3, 10, (1, 0, 1), False, False, id='3-10-pattern2-no_tensile'),
+    # 3-D n = 9: every axis pattern in row-major order, two of them along the Z-curve
+    pytest.param(3, 9, (1, 1, 1), True, False, id='3-9-pattern1'),
+    pytest.param(3, 9, (1, 0, 1), True, False, id='3-9-pattern2'),
+    pytest.param(3, 9, (0, 1, 0), True, False, id='3-9-pattern3'),
+    pytest.param(3, 9, (1, 1, 1), True, True, id='3-9-pattern1-zorder'),
+    pytest.param(3, 9, (0, 1, 0), True, True, id='3-9-pattern3-zorder')])
+def test_periodic_wcsph_steps_vs_oracle(gpu_device, dim, n, pattern, tensile, zorder):
+    periodic_wcsph_steps_vs_oracle(gpu_device, dim, n, pattern, tensile, zorder)
 
 
 # (test_library_on_cpu.py runs this on the library emulation; tensile is on unless it says not)
-def periodic_wcsph_steps_vs_oracle(gpu_device, dim, n, pattern, tensile=True):
+def periodic_wcsph_steps_vs_oracle(gpu_device, dim, n, pattern, tensile=True, zorder=False):
     """5 EPEC steps (continuity + momentum + AV + tensile + XSPH + Tait) in a
-    box periodic along `pattern`, against the ghost-materialising oracle.  Without
-    the tensile correction every pair pass takes the 32-byte records."""
+    box periodic along `pattern`, against the ghost-materialising oracle: the first
+    evaluation's pair count, accelerations, dt terms, p and cs, then the state.
+    Without the tensile correction every pair pass takes the 32-byte records;
+    zorder orders the cell rows along the Z-curve (B200SPH_ZORDER=1)."""
     import pysph_b200 as pb
     pa, params = _periodic_case(dim, n, tensile=tensile)
     ref_pa, _ = _periodic_case(dim, n, tensile=tensile)
@@ -157,17 +165,22 @@ def periodic_wcsph_steps_vs_oracle(gpu_device, dim, n, pattern, tensile=True):
                           periodic_in_x=bool(pattern[0]),
                           periodic_in_y=bool(pattern[1]),
                           periodic_in_z=bool(pattern[2]))
-    s = pb.make_wcsph_solver([pa], dict(params), pb.CubicSpline(dim=dim), domain=dm)
+    with pytest.MonkeyPatch.context() as mp:
+        mp.setenv('B200SPH_ZORDER', '1' if zorder else '0')
+        s = pb.make_wcsph_solver([pa], dict(params), pb.CubicSpline(dim=dim), domain=dm)
     o = orc.WCSPHOracleSolver([ref_pa], dict(params), 'CubicSpline',
                               domain=_dom_tuple(dm))
+    s.a_eval.count_pairs = True
     s.initialise()
     o.initialise()
+    assert s.a_eval.last_pairs == o.pairs_last_eval
+    s.a_eval.count_pairs = False
     s.pull()
     r = o.pas[0]
     nr = r.num_real_particles
     order = np.argsort(pa.gid)
     assert np.array_equal(r.gid[:nr], np.arange(nr))
-    for k in ('au', 'av', 'aw', 'arho', 'ax', 'ay', 'az'):
+    for k in ACC_FIELDS + ['p', 'cs']:
         ref = r.properties[k][:nr]
         if np.max(np.abs(ref)) == 0.0:
             assert np.max(np.abs(pa.properties[k])) == 0.0

@@ -1,8 +1,7 @@
 """Elastic-dynamics kernels (SURVEY.md 8f-2, BASELINE configs[4]): `k_solid_pass1/2` and
 `k_stage_solid` against the reference-generated goldens and the oracle, which IS pinned to
 the reference (tests/test_oracle_golden.py: test_elastic_dynamics_matches_reference_bodies).
-Also run against the host emulation of the whole library (tests/test_library_on_cpu.py) and
-with the kernel source compiled for the host (tests/test_kernel_source_on_cpu.py)."""
+Also run against the host emulation of the whole library (tests/test_library_on_cpu.py)."""
 import numpy as np
 import pytest
 
@@ -69,7 +68,8 @@ def test_solid_mech_step_matches_reference_bodies(gpu_device):
         for k, v in g['outputs'][key].items():
             if k in ('e', 'e0', 'ae'):
                 continue                  # not mirrored on the device (no energy equation)
-            assert np.allclose(pa.properties[k], v, rtol=0, atol=1e-6), (key, k)
+            # accelerations are fp32 on the device: 6e-8 of |a| * dt
+            assert np.allclose(pa.properties[k], v, rtol=0, atol=1e-7), (key, k)
 
 
 def test_rings_steps_vs_oracle(gpu_device):

@@ -31,7 +31,7 @@ def _build():
     import transform
     os.makedirs(BUILD, exist_ok=True)
     from pysph_b200 import build as lib_build
-    cpp = os.path.join(BUILD, 'b200sph_emul.cpp')
+    cpp = os.path.join(BUILD, 'b200sph_emulated.cpp')
     text, modes = transform.transform(lib_build.read_source())
     assert modes['k_list_build'] == 'emu::BLOCK' and modes['k_pair_list'] == 'emu::WARP' \
         and modes['k_stage'] == 'emu::SEQ' and modes['k_stage_pack'] == 'emu::BLOCK'
@@ -119,6 +119,9 @@ FAST = [
      {'dim': 2, 'n': 24, 'pattern': (1, 1, 0), 'tensile': False}),
     ('test_gpu_periodic', 'periodic_wcsph_steps_vs_oracle',
      {'dim': 3, 'n': 10, 'pattern': (1, 0, 1), 'tensile': False}),
+] + [('test_gpu_periodic', 'periodic_wcsph_steps_vs_oracle', {'dim': 3, 'n': 9, 'pattern': pat, 'zorder': z})
+     for pat, z in (((1, 1, 1), False), ((1, 0, 1), False), ((0, 1, 0), False), ((1, 1, 1), True),
+                    ((0, 1, 0), True))
 ] + [('test_gpu_edac', 'test_edac_evaluation_matches_reference_bodies', {'idx': i}) for i in range(4)] + [
     ('test_gpu_edac', 'test_edac_tvf_step_matches_reference_bodies', {}),
     ('test_gpu_edac', 'test_taylor_green_steps_vs_oracle', {'dim': 2, 'nx': 32, 'kernel': 'QuinticSpline'}),
