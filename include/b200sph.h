@@ -243,7 +243,9 @@ int b200sph_pull_u32(b200sph_ctx *ctx, int arr, int prop, uint32_t *host,
  * b200sph_synchronize.  Default off: every push/pull call is synchronous. */
 int b200sph_set_async_copies(b200sph_ctx *ctx, int on);
 /* device pointer of a property region of one array (for zero-copy use by
- * torch / NCCL plumbing); fp64 props -> double*, fp32 props -> float* */
+ * torch / NCCL plumbing); fp64 props -> double*, fp32 props -> float*.
+ * The pointers of x .. rho and x0 .. rho0 hold until the next stage call: a stage 1 may
+ * exchange the buffers behind the two sets of names instead of copying one into the other. */
 int b200sph_device_ptr(b200sph_ctx *ctx, int arr, int prop, void **out);
 
 /* ---- NNPS: kernel choice, DomainManager.update, NNPS.update ------------- */

@@ -237,6 +237,9 @@ struct b200sph_ctx {
     ArrayInfo arr[B200SPH_MAX_ARRAYS];
     int64_t pool_cap = 0;   // allocated particles in the pool
     int64_t pool_end = 0;   // off[last] + cap[last]
+    // by property id.  Which buffer goes by x .. rho and which by x0 .. rho0 changes when a fused
+    // stage 1 takes the initialize by renaming (init_by_rename): read these at enqueue time, and
+    // keep no copy of them across a stage
     double *f64[N_F64] = {nullptr};
     float *f32[N_F32] = {nullptr};
     uint32_t *u32[N_U32] = {nullptr};
@@ -685,6 +688,18 @@ static void **pool_buf(b200sph_ctx *ctx, int k, size_t *esz)
 static bool lists_usable(const b200sph_ctx *ctx, int64_t n) { return ctx->force_kernel == 0 && n < (1LL << LIST_JBITS); }
 // the current build's sorted order and lists can serve a light update
 static bool reusable_build(const b200sph_ctx *ctx) { return ctx->force_kernel == 0 && ctx->lists_valid && !ctx->topo_dirty; }
+// the fused stage `which` (it steps every array) may take a pending initialize by exchanging
+// the buffers x .. rho and x0 .. rho0 instead of copying one into the other: the stepped state
+// then exists in the new x .. rho only where this launch writes it, so every particle must be
+// one it steps -- no ghosts -- and it must not read the current state beside the stage copies,
+// which TVD-RK3's stages 2 and 3 do
+static bool init_by_rename(const b200sph_ctx *ctx, int which)
+{
+    if (which != 1) return false;
+    for (int a = 0; a < ctx->narr; a++)
+        if (ctx->arr[a].n != ctx->arr[a].n_real) return false;
+    return true;
+}
 
 // (re)build the pool so that every array owns [off, off+cap); moves existing data.
 static int pool_layout(b200sph_ctx *ctx, const int64_t *new_cap)
@@ -964,11 +979,16 @@ template <class S> static void stage_args(b200sph_ctx *ctx, S &sa, int arr, int 
 // ---- the deferred initialize ----------------------------------------------------------------
 // WCSPHStep.initialize of every array (WCSPHTVDRK3Step's is the same) copies x .. rho into
 // x0 .. rho0.  When the stage that follows will be the fused kernel, stage_impl only records it
-// (init_pending) and that kernel copies as it goes (do_init): one sweep over the state less per
-// step.  The one rule: whatever could observe the copy not being made yet -- reads x0 .. rho0,
+// (init_pending) and that kernel takes it as it goes (do_init): one sweep over the state less per
+// step.  Stage 1 of a context without ghosts does not even copy: the host exchanges the two sets
+// of buffers in ctx->f64 (init_by_rename), so that the state the initialize saw goes by
+// x0 .. rho0 where it lies and the kernel writes the stepped state into the buffers that now go
+// by x .. rho (INIT_RENAMED); 56 B per particle less to write.  Otherwise the kernel copies
+// (INIT_COPY).  The one rule: whatever could observe the copy not being made yet -- reads x0 .. rho0,
 // writes x .. rho, applies EOS calls to the pool's rho (eos_flush, pack_state), changes the
 // particle set or the stream -- runs it here first, as k_stage(0) on the state as it is, which is
 // the state the initialize saw.  ensure_pool does so for every entry point outside the fast path.
+// Only the fused stage 1 renames; every other way to the initialize copies.
 static int init_materialise(b200sph_ctx *ctx)
 {
     if (!ctx->init_pending) return 0;
@@ -2962,6 +2982,11 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
         return 0;
     }
     PhaseTimer pt(ctx, 2);
+    int do_init = ctx->init_pending ? INIT_COPY : INIT_NONE;
+    if (which != 0 && fused && ctx->init_pending && init_by_rename(ctx, which)) {
+        for (int k = 0; k <= B200SPH_RHO - B200SPH_X; k++) std::swap(ctx->f64[B200SPH_X + k], ctx->f64[B200SPH_X0 + k]);
+        do_init = INIT_RENAMED;
+    }
     StageArgs sa;
     stage_args(ctx, sa, arr, which, dt, devdt);
     if (rk3) sa.f = dt;   // every TVD-RK3 stage takes the whole dt
@@ -2975,12 +3000,16 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
         q.rank = ctx->rank; q.key_of = ctx->key_of;
         q.A0 = ctx->A0; q.AB = ctx->AB; q.C = ctx->C;
         q.R = ctx->rec32 ? ctx->R : nullptr;   // the layout the last pair pass read
+        if (q.R && ctx->hm_known && !std::isnan(ctx->h_uniform)) {   // 8 B per particle less to read
+            q.h = nullptr;
+            q.h_uniform = ctx->h_uniform;
+        }
         q.E32 = ctx->rec32_eos;
         q.G = ctx->G;
         q.red_u32 = ctx->red_u32;
         q.dt_cfl = f32_ptr(ctx, B200SPH_DT_CFL); q.dt_force = f32_ptr(ctx, B200SPH_DT_FORCE);
         q.red = ctx->red;
-        q.do_init = ctx->init_pending ? 1 : 0;
+        q.do_init = do_init;
         q.reduce_dt = (which == last && ctx->dt_adaptive_seen) ? 1 : 0;
         q.eos_any = ctx->eos_last_valid ? 1 : 0;
         q.E = ctx->eos_last;

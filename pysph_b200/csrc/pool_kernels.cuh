@@ -250,7 +250,8 @@ __device__ __forceinline__ void eos_tab_apply(double *__restrict__ rho, float *_
 // k_stage_pack, or with WCSPHTVDRK3Step: k_stage_pack_rk3; the neighbour lists of the current
 // build are reusable): in ONE pass over the pool, per real particle,
 //   [initialize (integrator_step.py:51-61) when it was deferred to here: the copies take the
-//    rho of before the EOS calls below, as the reference's initialize, which runs before them]
+//    rho of before the EOS calls below, as the reference's initialize, which runs before them;
+//    with INIT_RENAMED there is nothing to copy, x0 .. rho0 are that state already]
 //   [the pool side of the last evaluation's EOS calls (k_eos_tab's arithmetic) when the pair
 //    pass left it to here: rho clamp, p, cs -- ghosts included, as k_eos_tab]
 //   stage1 / stage2 (integrator_step.py:63-91), fp64, wcsph_combine as k_stage
@@ -267,8 +268,14 @@ __device__ __forceinline__ void eos_tab_apply(double *__restrict__ rho, float *_
 // (+ k_reduce_dt): six sweeps over the fp64 state become one.  Ghost particles are not stepped
 // (integrator_cython.mako:97-111) and their records are refreshed by the halo scatter.
 // ---------------------------------------------------------------------------
+// how the launch takes a deferred initialize (init_materialise): there is none; it copies
+// x .. rho into x0 .. rho0 as it goes; or the host renamed the buffers (init_by_rename), so
+// that a.x0 .. a.rho0 are the state before the stage and a.x .. a.rho only receive the new one
+enum { INIT_NONE = 0, INIT_COPY = 1, INIT_RENAMED = 2 };
+
 struct FusePackArgs {
-    const double *h, *m;
+    const double *h, *m;             // h null: every particle has h_uniform (the 32-byte records need that)
+    double h_uniform;
     float *p, *cs;                   // pool values: read for arrays without a speculated EOS, written by EP
     const uint32_t *rank, *key_of;   // pool index -> sorted slot / cell key of the current build
     const float4 *A0;                // packed positions at build time (sorted order)
@@ -279,7 +286,7 @@ struct FusePackArgs {
     unsigned *red_u32;
     const float *dt_cfl, *dt_force;
     long long *red;
-    int do_init, reduce_dt, eos_any;
+    int do_init, reduce_dt, eos_any; // do_init: INIT_*
     EosTab E;
     int eos_pool;                    // apply EP to the pool's rho / p / cs first
     EosTab EP;
@@ -295,8 +302,11 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
     float d2 = 0.f, dh = 0.f;
     double mc = -1e300, mf = -1e300, hm = 1e300;
     const uint8_t t = g < a.pool_end ? a.ptype[g] : (uint8_t)PT_INVALID;
+    // (with the type, not behind it: one round trip to memory less before A0[s] can be asked for;
+    // both arrays have a slot for every slot of the pool)
+    const uint32_t s = g < a.pool_end ? q.rank[g] : 0u, key = g < a.pool_end ? q.key_of[g] : 0u;
     if (t != PT_INVALID) {
-        const double hg = q.h[g];
+        const double hg = q.h ? q.h[g] : q.h_uniform;
         hm = hg;
         if (t & PT_GHOST) {
             if (q.eos_pool) eos_tab_apply(a.rho, q.p, q.cs, t, g, q.EP);
@@ -306,21 +316,21 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
             // the EOS calls clamps it; the stage overwrites the pool's rho, so only TVD-RK3's
             // stages 2 and 3 read the clamped value
             const bool eos = q.eos_pool && eos_tab_applies(q.EP, t);
-            double rc = 0.0;
-            if (q.do_init || eos || (RK3 && a.which != 1)) rc = a.rho[g];
             double x0, y0, z0, u0, v0, w0, r0;
-            if (q.do_init) {
+            if (q.do_init == INIT_COPY) {
                 x0 = a.x[g]; y0 = a.y[g]; z0 = a.z[g];
                 u0 = a.u[g]; v0 = a.v[g]; w0 = a.w[g];
-                r0 = rc;
+                r0 = a.rho[g];
                 a.x0[g] = x0; a.y0[g] = y0; a.z0[g] = z0;
                 a.u0[g] = u0; a.v0[g] = v0; a.w0[g] = w0;
                 a.rho0[g] = r0;
-            } else {
+            } else {   // (INIT_RENAMED: the state the initialize saw already goes by x0 .. rho0)
                 x0 = a.x0[g]; y0 = a.y0[g]; z0 = a.z0[g];
                 u0 = a.u0[g]; v0 = a.v0[g]; w0 = a.w0[g];
                 r0 = a.rho0[g];
             }
+            double rc = r0;
+            if (q.do_init == INIT_NONE && (eos || (RK3 && a.which != 1))) rc = a.rho[g];
             float p_eos = 0.f, cs_eos = 0.f;
             if (eos) {
                 eos_tab_eval(q.EP, t & 7, rc, p_eos, cs_eos);
@@ -353,8 +363,7 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
                 mf = (double)q.dt_force[g];
             }
             // ---- records of the next evaluation ---------------------------------------
-            const uint32_t s = q.rank[g];
-            const float4 A = pack_position(q.G, q.key_of[g], xn, yn, zn, hg);
+            const float4 A = pack_position(q.G, key, xn, yn, zn, hg);
             const int ar = t & 7;
             if (q.R) {
                 // only the full sector: a lone 16-byte half would cost a read-modify-write in
@@ -428,7 +437,7 @@ __global__ void __launch_bounds__(256, 4) k_stage_pack(const StageArgs a, const 
 }
 
 // k_stage_pack for WCSPHTVDRK3Step (which = 1, 2, 3; dt is used whole): stages 2 and 3 read
-// the current state as well as the stage copies.  61 registers, no spills at 4 CTAs/SM.
+// the current state as well as the stage copies.  62 registers, no spills at 4 CTAs/SM.
 __global__ void __launch_bounds__(256, 4) k_stage_pack_rk3(const StageArgs a, const FusePackArgs q)
 {
     __shared__ float s_d2[8], s_dh[8];
