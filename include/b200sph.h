@@ -356,6 +356,37 @@ enum {
 int b200sph_density_filter(b200sph_ctx *ctx, uint32_t array_mask, int mode, int kernel, int rhotmp_prop,
                            int real_only);
 
+/* ---- interpolation at probe points: Interpolator (pysph/tools/interpolator.py:18-510) -------
+ * b200sph_probe_create: n points (x, y, z, host fp64, copied) with the probes' smoothing length h
+ *   (the Interpolator's: the largest h of its arrays when the points were set).  Returns the id
+ *   (>= 0) of a device-resident probe set; several may live on one context.
+ * b200sph_probe_release: frees the set `id`.
+ * b200sph_interpolate: the property of every source particle -- the particles of the arrays in
+ *   array_mask, ghosts included -- interpolated at the probes of `id` with `method`
+ *   (B200SPH_INTERP_*) and smoothing kernel `kernel` (B200SPH_KERNEL_*) in `dim` dimensions (the
+ *   Interpolator's, not the context's).  props[a] (B200SPH_MAX_ARRAYS entries) is the property id
+ *   to read for array a, any floating-point or user property; -1: the array lacks the property
+ *   (it contributes f = 0 and its weights).  out: n values, for ORDER1 4 n (value, d/dx, d/dy,
+ *   d/dz per probe; components beyond dim are 0, and all four are 0 where gj_solve returns early).
+ *   ORDER1's SummationDensity goes to a scratch buffer: the pool's rho is never written.
+ *   Read-only: it walks the cells of the last neighbour-search build around each probe, wide
+ *   enough for the kernel's reach and for the drift of the particles since that build (measured
+ *   on the device in the same call), and never rebuilds the lists or moves the solver's schedule.
+ *   Waits for its result.  Refused: the slab decomposition; a particle set changed since the last
+ *   nnps_update; a stencil that would visit a cell of a periodic axis twice (2 R + 1 > nc).
+ * New symbols only: B200SPH_ABI_VERSION stays 5. */
+enum {
+    B200SPH_INTERP_SHEPARD = 0,      /* InterpolateFunction                        */
+    B200SPH_INTERP_SPH = 1,          /* InterpolateSPH                             */
+    B200SPH_INTERP_SPLASH = 2,       /* SPLASHInterpolateProperty                  */
+    B200SPH_INTERP_SPLASH_NORM = 3,  /* SPLASHInterpolatePropertyNormalized        */
+    B200SPH_INTERP_ORDER1 = 4        /* SummationDensity, SPHFirstOrderApproximation(PreStep) */
+};
+int b200sph_probe_create(b200sph_ctx *ctx, int64_t n, const double *x, const double *y, const double *z, double h);
+int b200sph_probe_release(b200sph_ctx *ctx, int id);
+int b200sph_interpolate(b200sph_ctx *ctx, int id, int method, int kernel, int dim, const int *props,
+                        uint32_t array_mask, double *out);
+
 /* The two Groups of EDACScheme._get_internal_flow_equations (wc/edac.py:776-880) in
  * the generated AccelerationEval.compute (acceleration_eval_cython.mako:10-154): group 1 computes
  * V = sum W, rho = m V (transport_velocity.py:24-58) and the neighbour-average

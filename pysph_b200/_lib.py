@@ -53,6 +53,9 @@ EQ_LAMINAR = 32
 # density re-initialisation filters (B200SPH_DFILTER_*)
 DFILTER_SHEPARD, DFILTER_MLS2D, DFILTER_MLS3D = 0, 1, 2
 
+# interpolation methods (B200SPH_INTERP_*), by the Interpolator's method names
+INTERP_METHODS = {'shepard': 0, 'sph': 1, 'splash': 2, 'splash_norm': 3, 'order1': 4}
+
 HALO_FIELDS = 9
 MIGRATE_FIELDS = 17
 HALO_FIELD_NAMES = ('x', 'y', 'z', 'u', 'v', 'w', 'rho', 'h', 'm')
@@ -158,6 +161,10 @@ SIGNATURES = {
     'b200sph_generic_launch': (C.c_int, [_ctx_p, C.c_int, C.c_char_p, C.c_int, C.c_int, C.c_uint,
                                          C.c_int, C.c_double, C.c_double, C.c_int]),
     'b200sph_density_filter': (C.c_int, [_ctx_p, C.c_uint32, C.c_int, C.c_int, C.c_int, C.c_int]),
+    'b200sph_probe_create': (C.c_int, [_ctx_p, _i64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double]),
+    'b200sph_probe_release': (C.c_int, [_ctx_p, C.c_int]),
+    'b200sph_interpolate': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int),
+                                      C.c_uint32, C.c_void_p]),
     'b200sph_tvf_pass': (C.c_int, [_ctx_p, C.POINTER(TvfProgram), C.POINTER(_i64)]),
     'b200sph_stage_tvf': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_double]),
     'b200sph_stage_tvf_dev': (C.c_int, [_ctx_p, C.c_int, C.c_int]),

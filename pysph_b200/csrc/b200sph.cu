@@ -21,7 +21,8 @@
 //
 // One translation unit: this file holds the context, the pool and every C-ABI entry
 // point; the kernels are included below by family (pool_kernels, scan, nnps_kernels,
-// sph_kernels, pair_kernel, pair_list, tvf_kernels, solid_kernels, halo_kernels .cuh).
+// sph_kernels, pair_kernel, pair_list, tvf_kernels, solid_kernels, halo_kernels, density_filter,
+// interp_kernels .cuh).
 //
 // No CPU fallback: every entry point needs a CUDA device.
 #include "b200sph.h"
@@ -401,6 +402,17 @@ struct b200sph_ctx {
     // density_filter: its records, [2 n_sorted] (allocated on first use)
     float4 *dfilter_F = nullptr;
     size_t dfilter_cap = 0;
+    // interpolation (b200sph_probe_*, b200sph_interpolate): the probe sets by id (xyz: 3 n doubles,
+    // null once released), the records [2 n_sorted] and order1's rho [n_sorted], the reach
+    // reduction and the results (allocated on first use)
+    struct ProbeSet { double *xyz = nullptr; int64_t n = 0; double h = 0.0; };
+    std::vector<ProbeSet> probes;
+    float4 *interp_Q = nullptr;
+    float *interp_rho = nullptr;
+    size_t interp_cap = 0;
+    unsigned *interp_red = nullptr;
+    double *interp_out = nullptr;
+    size_t interp_out_cap = 0;
     // Group(start_idx, stop_idx): one-shot destination ranges of the next pair pass
     int64_t dst_lo[B200SPH_MAX_ARRAYS] = {0}, dst_hi[B200SPH_MAX_ARRAYS] = {0};
     bool dst_ranged = false;
@@ -646,6 +658,7 @@ __device__ __forceinline__ void rec32_make(const float4 A, const double u, const
 #include "solid_kernels.cuh"
 #include "halo_kernels.cuh"
 #include "density_filter.cuh"
+#include "interp_kernels.cuh"
 
 // --------------------------------------------------------------------------
 // host side
@@ -1113,6 +1126,8 @@ int b200sph_destroy(b200sph_ctx *ctx)
     generic_unload_all(ctx);
     for (int k = 0; k < N_F32X; k++) cudaFree(ctx->f32x[k]);
     cudaFree(ctx->Dv); cudaFree(ctx->PT); cudaFree(ctx->dfilter_F);
+    for (auto &ps : ctx->probes) cudaFree(ps.xyz);
+    cudaFree(ctx->interp_Q); cudaFree(ctx->interp_rho); cudaFree(ctx->interp_red); cudaFree(ctx->interp_out);
     for (auto &sg : ctx->mirror_segs) cudaFree(sg.idx);
     for (int k = 0; k < 12; k++) cudaFree(ctx->f64s[k]);
     for (int k = 0; k < 21; k++) cudaFree(ctx->f32s[k]);
@@ -2453,6 +2468,151 @@ int b200sph_density_filter(b200sph_ctx *ctx, uint32_t array_mask, int mode, int 
     // rho changed: the next evaluation packs its records (and applies its EOS) from it
     state_changed(ctx);
     ctx->spec_records = false;
+    return 0;
+}
+
+// ---- Interpolator (interp_kernels.cuh) ----------------------------------------------------------
+int b200sph_probe_create(b200sph_ctx *ctx, int64_t n, const double *x, const double *y, const double *z, double h)
+{
+    CU(cudaSetDevice(ctx->device));
+    if (n < 0 || (n > 0 && (!x || !y || !z))) return set_err(ctx, "probe_create: bad points (n = %lld)", (long long)n);
+    if (!(h > 0.0) || !std::isfinite(h)) return set_err(ctx, "probe_create: the probes' smoothing length must be > 0 (got %g)", h);
+    b200sph_ctx::ProbeSet ps;
+    ps.n = n;
+    ps.h = h;
+    if (n > 0) {
+        CU(cudaMalloc((void **)&ps.xyz, 24 * (size_t)n));
+        for (int d = 0; d < 3; d++)
+            CU(cudaMemcpyAsync(ps.xyz + d * n, d == 0 ? x : (d == 1 ? y : z), 8 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+    }
+    for (size_t i = 0; i < ctx->probes.size(); i++)
+        if (ctx->probes[i].n < 0) {
+            ctx->probes[i] = ps;
+            return (int)i;
+        }
+    ctx->probes.push_back(ps);
+    return (int)ctx->probes.size() - 1;
+}
+
+int b200sph_probe_release(b200sph_ctx *ctx, int id)
+{
+    if (id < 0 || id >= (int)ctx->probes.size() || ctx->probes[id].n < 0) return set_err(ctx, "probe_release: no probe set %d", id);
+    CU(cudaSetDevice(ctx->device));
+    CU(cudaStreamSynchronize(ctx->stream));
+    if (ctx->probes[id].xyz) CU(cudaFree(ctx->probes[id].xyz));
+    ctx->probes[id] = b200sph_ctx::ProbeSet();
+    ctx->probes[id].n = -1;   // a free slot
+    return 0;
+}
+
+// A reader like pull_f64: the pending EOS calls are applied first, nothing the time loop caches
+// is invalidated, and the only state it leaves behind is its own scratch.  It needs the build's
+// sorted order to hold the current particle set, not its lists or a fresh grid: the stencil
+// covers the drift since the build, measured in k_interp_pack.
+int b200sph_interpolate(b200sph_ctx *ctx, int id, int method, int kernel, int dim, const int *props, uint32_t array_mask,
+                        double *out)
+{
+    if (int rcc = require_confirmed(ctx, "interpolate")) return rcc;
+    CU(cudaSetDevice(ctx->device));
+    int rc = ensure_pool(ctx);
+    if (rc) return rc;
+    if (id < 0 || id >= (int)ctx->probes.size() || ctx->probes[id].n < 0) return set_err(ctx, "interpolate: no probe set %d", id);
+    if (method < B200SPH_INTERP_SHEPARD || method > B200SPH_INTERP_ORDER1) return set_err(ctx, "interpolate: unknown method %d", method);
+    if (kernel < 0 || kernel > 3) return set_err(ctx, "interpolate: unknown kernel id %d", kernel);
+    if (dim < 1 || dim > 3) return set_err(ctx, "interpolate: dim must be 1, 2 or 3 (got %d)", dim);
+    if (kernel == B200SPH_KERNEL_WENDLAND_QUINTIC && dim == 1) return set_err(ctx, "WendlandQuintic: Dim 1 not supported");
+    if (array_mask == 0 || array_mask >= (1u << ctx->narr)) return set_err(ctx, "interpolate: bad array mask 0x%x", array_mask);
+    if (!props) return set_err(ctx, "interpolate: no property ids");
+    if (ctx->peer_box || ctx->comm_pending)
+        return set_err(ctx, "interpolate runs on one GPU (no slab decomposition: a probe near a cut needs the other rank's particles)");
+    InterpArgs ia;
+    memset(&ia, 0, sizeof(ia));
+    for (int a = 0; a < ctx->narr; a++) {
+        const int p = props[a];
+        if (p == -1 || !((array_mask >> a) & 1u)) continue;
+        if (is_f64_prop(p) && (!is_solid_prop(p) || ctx->solid_alloc) && f64_ptr(ctx, p)) ia.fd[a] = f64_ptr(ctx, p);
+        else if (is_f32_prop(p) && (p < B200SPH_V00 || ctx->solid_alloc) && f32_ptr(ctx, p)) ia.ff[a] = f32_ptr(ctx, p);
+        else return set_err(ctx, "interpolate: property id %d (array %d) is not a floating-point property of the pool", p, a);
+    }
+    int64_t ntot = 0;
+    for (int a = 0; a < ctx->narr; a++) ntot += ctx->arr[a].n;
+    if (ctx->topo_dirty || ctx->n_sorted != ntot)
+        return set_err(ctx, "interpolate: the particle set changed since the last neighbour-search build; call nnps_update first");
+    const b200sph_ctx::ProbeSet &ps = ctx->probes[id];
+    const double kr = kernel_radius_scale(kernel);
+    // the stencil without the drift already visits a periodic cell twice
+    for (int d = 0; d < 3; d++)
+        if (ctx->G.periodic[d] && ntot > 0) {
+            const int R = (int)std::ceil(kr * ps.h / ctx->G.cell[d]);
+            if (2 * R + 1 > ctx->G.nc[d])
+                return set_err(ctx, "interpolate: the stencil (%d cells) wraps onto itself along periodic axis %d (%d cells): "
+                                    "the kernel's reach %g is too large for the box", 2 * R + 1, d, ctx->G.nc[d], kr * ps.h);
+        }
+    const size_t nout = (size_t)ps.n * (method == B200SPH_INTERP_ORDER1 ? 4 : 1);
+    if (ps.n == 0) return 0;
+    if (ntot == 0) {
+        memset(out, 0, 8 * nout);
+        return 0;
+    }
+    if ((rc = eos_flush(ctx))) return rc;
+    if ((size_t)ctx->n_sorted > ctx->interp_cap) {
+        if (ctx->interp_Q) CU(cudaFree(ctx->interp_Q));
+        if (ctx->interp_rho) CU(cudaFree(ctx->interp_rho));
+        ctx->interp_Q = nullptr, ctx->interp_rho = nullptr;
+        CU(cudaMalloc((void **)&ctx->interp_Q, 2 * sizeof(float4) * (size_t)ctx->n_sorted));
+        CU(cudaMalloc((void **)&ctx->interp_rho, sizeof(float) * (size_t)ctx->n_sorted));
+        ctx->interp_cap = (size_t)ctx->n_sorted;
+    }
+    if (!ctx->interp_red) CU(cudaMalloc((void **)&ctx->interp_red, 8 * sizeof(unsigned)));
+    if (nout > ctx->interp_out_cap) {
+        if (ctx->interp_out) CU(cudaFree(ctx->interp_out));
+        ctx->interp_out = nullptr;
+        CU(cudaMalloc((void **)&ctx->interp_out, 8 * nout));
+        ctx->interp_out_cap = nout;
+    }
+    {
+        PhaseTimer pt(ctx, 2);
+        ia.x = ctx->f64[B200SPH_X]; ia.y = ctx->f64[B200SPH_Y]; ia.z = ctx->f64[B200SPH_Z];
+        ia.h = ctx->f64[B200SPH_H]; ia.m = ctx->f64[B200SPH_M]; ia.rho = ctx->f64[B200SPH_RHO];
+        ia.perm = ctx->perm; ia.skey = ctx->skey; ia.cell_start = ctx->cell_start; ia.stype = ctx->stype;
+        ia.n = ctx->n_sorted;
+        ia.G = ctx->G;
+        ia.Q = ctx->interp_Q; ia.rho_sph = ctx->interp_rho; ia.red = ctx->interp_red;
+        ia.mask = array_mask;
+        ia.px = ps.xyz; ia.py = ps.xyz + ps.n; ia.pz = ps.xyz + 2 * ps.n;
+        ia.np = ps.n;
+        ia.hp = (float)ps.h;
+        ia.k = (float)kr;
+        ia.kfac = (float)kernel_fac(kernel, dim);
+        ia.method = method;
+        ia.out = ctx->interp_out;
+        CU(cudaMemsetAsync(ctx->interp_red, 0, 8 * sizeof(unsigned), ctx->stream));
+        k_interp_pack<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(ia);
+        LAUNCH_CHECK();
+        const unsigned nbp = (unsigned)cdiv(ps.n * 32, INTERP_NT);
+        const unsigned nbd = (unsigned)cdiv(ctx->n_sorted * 32, INTERP_NT);
+        rc = with_kernel_dim(ctx, kernel, dim, "interpolate", [&](auto kc, auto dc) {
+            constexpr int K = decltype(kc)::value, D = decltype(dc)::value;
+            if (method == B200SPH_INTERP_ORDER1) {
+                k_interp_density<K, D><<<nbd, INTERP_NT, 0, ctx->stream>>>(ia);
+                LAUNCH_CHECK();
+                k_interp<K, D, true><<<nbp, INTERP_NT, 0, ctx->stream>>>(ia);
+            } else {
+                k_interp<K, D, false><<<nbp, INTERP_NT, 0, ctx->stream>>>(ia);
+            }
+            LAUNCH_CHECK();
+            return 0;
+        });
+        if (rc) return rc;
+    }
+    unsigned wrapped = 0;
+    CU(cudaMemcpyAsync(out, ctx->interp_out, 8 * nout, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(&wrapped, ctx->interp_red + 4, sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    if (wrapped)
+        return set_err(ctx, "interpolate: the stencil wraps onto itself along a periodic axis: the kernel's reach plus the "
+                            "drift since the last neighbour-search build spans the box; call nnps_update first");
     return 0;
 }
 
