@@ -32,7 +32,7 @@ extern "C" {
 #define B200SPH_MAX_ARRAYS 8
 #define B200SPH_MAX_USER 16    /* user properties of the generic-equation fallback */
 #define B200SPH_MAX_RANKS 16   /* ranks of one node in the peer protocol (b200sph_peer_*) */
-#define B200SPH_ABI_VERSION 5
+#define B200SPH_ABI_VERSION 6
 
 typedef struct b200sph_ctx b200sph_ctx;
 
@@ -347,7 +347,7 @@ int b200sph_generic_launch(b200sph_ctx *ctx, int module, const char *kernel, int
  * rho.  Refused: periodic or mirror domains, the slab decomposition, lists that cannot index
  * the particles, MLS2D with dim != 2 and MLS3D with dim != 3.
  * A new symbol only: no structure and no b200sph_stats counter changed, so
- * B200SPH_ABI_VERSION stays 5. */
+ * B200SPH_ABI_VERSION stayed 5. */
 enum {
     B200SPH_DFILTER_SHEPARD = 0,
     B200SPH_DFILTER_MLS2D = 1,
@@ -374,7 +374,7 @@ int b200sph_density_filter(b200sph_ctx *ctx, uint32_t array_mask, int mode, int 
  *   on the device in the same call), and never rebuilds the lists or moves the solver's schedule.
  *   Waits for its result.  Refused: the slab decomposition; a particle set changed since the last
  *   nnps_update; a stencil that would visit a cell of a periodic axis twice (2 R + 1 > nc).
- * New symbols only: B200SPH_ABI_VERSION stays 5. */
+ * New symbols only: B200SPH_ABI_VERSION stayed 5. */
 enum {
     B200SPH_INTERP_SHEPARD = 0,      /* InterpolateFunction                        */
     B200SPH_INTERP_SPH = 1,          /* InterpolateSPH                             */
@@ -452,7 +452,7 @@ int b200sph_stage_dev(b200sph_ctx *ctx, int arr, int which);
  * of b200sph_stage_dev (k_stage_pack_rk3, same conditions and results bitwise those of the
  * separate kernels), with the adaptive-dt factors reduced after stage3, the end of the step.
  * These two entries are new symbols only: no structure and no b200sph_stats counter changed,
- * so B200SPH_ABI_VERSION stays 5. */
+ * so B200SPH_ABI_VERSION stayed 5. */
 int b200sph_stage_rk3(b200sph_ctx *ctx, int arr, int which, double dt);
 /* the same with dt read from the device-resident time-control block */
 int b200sph_stage_rk3_dev(b200sph_ctx *ctx, int arr, int which);
@@ -501,7 +501,7 @@ int b200sph_halo_layout(b200sph_ctx *ctx, int *halo_fields, int *migrate_fields)
  * B200SPH_HALO_FIELDS doubles field-major and TIGHT (field f of particle k at
  * dev_buf[f * count + k]); *count = number selected; error if count > cap.
  * slot = 0 / 1 (left / right neighbour) also remembers the selection for
- * b200sph_halo_pack_selected; slot = -1 does not */
+ * b200sph_halo_pack_selected and b200sph_peer_send; slot = -1 does not */
 int b200sph_halo_pack(b200sph_ctx *ctx, int arr, int slot, double lo, double hi,
                       double *dev_buf, int64_t cap, int64_t *count);
 /* pack the CURRENT values of the particles remembered by the last
@@ -513,17 +513,6 @@ int b200sph_halo_pack_selected(b200sph_ctx *ctx, int arr, int slot, double *dev_
  * [ghost_first, ghost_first + n) of `arr` (indices among the ghosts) */
 int b200sph_halo_overwrite(b200sph_ctx *ctx, int arr, int64_t ghost_first,
                            const double *dev_buf, int64_t stride, int64_t n);
-/* the refresh message of ALL arrays for neighbour `slot` in one kernel: the block
- * of array a starts at 9 * (count_0 + .. + count_{a-1}) doubles, field-major and
- * tight.  dev_buf may be a PEER pointer obtained with b200sph_ipc_open (the
- * neighbour's staging buffer): pack and send are then the same kernel, writing
- * over NVLink */
-int b200sph_halo_pack_selected_all(b200sph_ctx *ctx, int slot, double *dev_buf,
-                                   int64_t cap_doubles, int64_t *ndoubles);
-/* the inverse on the receiving rank: counts[a] particles of array a (block
- * layout as above) over the existing ghosts starting at ghost_first[a] */
-int b200sph_halo_overwrite_all(b200sph_ctx *ctx, const int64_t *ghost_first,
-                               const int64_t *counts, const double *dev_buf);
 /* peer-memory staging buffers (ranks of one node): allocate + export a 64-byte
  * cudaIpcMemHandle_t / map a neighbour's buffer / unmap (owner = 0) or free (1) */
 int b200sph_ipc_alloc(b200sph_ctx *ctx, int64_t bytes, void **dev_ptr, void *handle64);
@@ -533,11 +522,6 @@ int b200sph_ipc_close(b200sph_ctx *ctx, void *dev_ptr, int owner);
  * current neighbour build (-1 if there is no reusable build), out[1] = the skin
  * S: the build can be reused while out[0] <= out[1] */
 int b200sph_nnps_drift(b200sph_ctx *ctx, double out[2]);
-/* the same measurement without a host round trip: writes out[0] / out[1] (the
- * fraction of the skin used up) to a DEVICE double, stream ordered, so that a
- * collective can reduce it directly.  Returns 1 (and writes nothing) if there is
- * no reusable build, 0 otherwise */
-int b200sph_nnps_drift_device(b200sph_ctx *ctx, double *dev_ratio);
 /* the caller decided (collectively, over all ranks) that the current build is
  * kept for the next nnps_update: that update then only refreshes the packed
  * positions and does not repeat the drift measurement (saves a host sync) */
@@ -561,16 +545,22 @@ int b200sph_nnps_keep_build(b200sph_ctx *ctx);
  *                 not, then let the communication stream wait for the main stream;
  *                 returns 1 if there is no reusable build (publish says so to everyone)
  *   peer_publish  {used-up fraction of the list skin, dt proposal | +inf} to every rank
- *   peer_send     b200sph_halo_pack_selected_all into the neighbour's staging buffer
- *                 (remote_staging: its buffer mapped with b200sph_ipc_open) + the
- *                 data-ready flag in its mailbox; side = 0: I am its RIGHT neighbour's
- *                 left... precisely: side is the slot the RECEIVER reads, 0 = message from
- *                 its left neighbour, 1 = from its right neighbour
+ *   peer_send     the ghost message for neighbour nb_rank, written over NVLink straight
+ *                 into its staging buffer (remote_staging: mapped with b200sph_ipc_open,
+ *                 cap_doubles long), then the data-ready flag in its mailbox.  The message
+ *                 holds the CURRENT values of the particles remembered by the last
+ *                 b200sph_halo_pack(arr, slot, ...) of every array: array a's block starts at
+ *                 nf * (count_0 + .. + count_{a-1}) doubles (nf: b200sph_halo_layout), field
+ *                 f of its particle k at f * count_a + k.  slot = -1 sends the flag alone
+ *                 (no reusable build).  side is the flag the RECEIVER reads: 0 = message
+ *                 from its left neighbour, 1 = from its right neighbour
  *   peer_reduce   wait for every rank's scalars: MAX fraction -> the decision (device,
  *                 and pinned host memory for peer_decision), MIN dt -> block[2]
- *   peer_recv     wait for the data-ready flag `side`, then b200sph_halo_overwrite_all
- *                 from the local staging buffer, including the ghosts' packed pair
- *                 records (position + state with the last evaluation's EOS calls)
+ *   peer_recv     wait for the data-ready flag `side`, then scatter the message in the
+ *                 local staging buffer (layout as in peer_send) over the existing ghosts:
+ *                 counts[a] particles of array a starting at its ghost ghost_first[a].  With
+ *                 a reusable build the ghosts' packed pair records are refreshed in the same
+ *                 pass (position + state with the last evaluation's EOS calls)
  *   peer_end      from here b200sph_pair_pass may run the destinations that do not
  *                 depend on ghosts while the above is still in flight; every other entry
  *                 point that touches particle data first waits for it

@@ -203,16 +203,11 @@ SIGNATURES = {
                                              _i64, C.POINTER(_i64)]),
     'b200sph_halo_overwrite': (C.c_int, [_ctx_p, C.c_int, _i64, C.c_void_p, _i64,
                                          _i64]),
-    'b200sph_halo_pack_selected_all': (C.c_int, [_ctx_p, C.c_int, C.c_void_p, _i64,
-                                                 C.POINTER(_i64)]),
-    'b200sph_halo_overwrite_all': (C.c_int, [_ctx_p, C.POINTER(_i64),
-                                             C.POINTER(_i64), C.c_void_p]),
     'b200sph_ipc_alloc': (C.c_int, [_ctx_p, _i64, C.POINTER(C.c_void_p),
                                     C.c_void_p]),
     'b200sph_ipc_open': (C.c_int, [_ctx_p, C.c_void_p, C.POINTER(C.c_void_p)]),
     'b200sph_ipc_close': (C.c_int, [_ctx_p, C.c_void_p, C.c_int]),
     'b200sph_nnps_drift': (C.c_int, [_ctx_p, _dp]),
-    'b200sph_nnps_drift_device': (C.c_int, [_ctx_p, C.c_void_p]),
     'b200sph_nnps_keep_build': (C.c_int, [_ctx_p]),
     'b200sph_halo_append': (C.c_int, [_ctx_p, C.c_int, C.c_void_p, _i64, _i64,
                                       C.c_int, C.c_int]),

@@ -277,7 +277,7 @@ struct b200sph_ctx {
     // grid
     b200sph_grid_info grid;
     bool grid_valid = false;
-    bool packed_valid = false;  // A / AB hold the CURRENT positions (set by nnps_drift_device, kept by halo_overwrite_all)
+    bool packed_valid = false;  // A / AB hold the CURRENT positions (set by a light update, the fused stage kernel or peer_begin; kept by peer_recv)
     double last_domain_size = 0.0;
 
     // sort / cell list buffers
@@ -527,7 +527,7 @@ static void pool_moved(b200sph_ctx *ctx)
     ctx->lists_valid = false;
 }
 
-// Ghost values were overwritten in place (halo_overwrite_all, peer_recv).  With a reusable
+// Ghost values were overwritten in place (peer_recv).  With a reusable
 // build whose packed positions are current, the same launch repacks the ghosts' positions
 // (`repacked`) and, `records`, their state records: those flags stay.
 static void ghosts_refreshed(b200sph_ctx *ctx, bool repacked, bool records)
@@ -1627,15 +1627,18 @@ int b200sph_update_domain(b200sph_ctx *ctx)
     return 0;
 }
 
-// 2 |dx|max + k dh <= S, with a 2 % safety margin for the fp32 measurement
-static bool drift_within_skin(b200sph_ctx *ctx, const unsigned *raw)
+// 2 |dx|max + k dh: the part of the skin the drift since the build has used up, in length
+// units, from a host copy of the fp32 max-reduction red_u32[0..1] (|dx|^2 and dh as bits)
+static double drift_need(const b200sph_ctx *ctx, const unsigned *raw)
 {
     float d2, dh;
     memcpy(&d2, &raw[0], 4);
     memcpy(&dh, &raw[1], 4);
-    const double need = 2.0 * std::sqrt((double)d2) + ctx->radius_scale * (double)dh;
-    return need <= 0.98 * ctx->S_abs;
+    return 2.0 * std::sqrt((double)d2) + ctx->radius_scale * (double)dh;
 }
+
+// 2 |dx|max + k dh <= S, with a 2 % safety margin for the fp32 measurement
+static bool drift_within_skin(b200sph_ctx *ctx, const unsigned *raw) { return drift_need(ctx, raw) <= 0.98 * ctx->S_abs; }
 
 // Skin controller, part 2 (part 1 adapts the skin geometrically from the lifetime of the build
 // that has just ended, see nnps_update).  A build is RETIRED -- rebuilt although it is valid --
@@ -1682,11 +1685,11 @@ static int nnps_light_update(b200sph_ctx *ctx)
 {
     if (ctx->n_sorted <= 0) return 1;
     if (ctx->drift_ok) {
-        // the drift was just measured by b200sph_nnps_drift (multi-GPU: the decision to
-        // keep the build is collective); only refresh the packed positions, no host sync
+        // the drift was just measured by b200sph_nnps_drift or peer_begin (multi-GPU: the
+        // decision to keep the build is collective); only refresh the packed positions, no host sync
         ctx->drift_ok = false;
         drift_consumed(ctx);
-        if (ctx->packed_valid) return 1;   // nnps_drift_device packed them, halo_overwrite_all kept the ghosts current
+        if (ctx->packed_valid) return 1;   // peer_begin packed them, peer_recv kept the ghosts current
         if (int rc = pack_positions_light(ctx, 0)) return rc;
         return 1;
     }
@@ -1715,13 +1718,8 @@ static int confirm_pending(b200sph_ctx *ctx, int *redo)
     CU(cudaSetDevice(ctx->device));
     CU(cudaEventSynchronize(ctx->drift_evt));
     ctx->check_pending = false;
-    {
-        float d2, dh;
-        memcpy(&d2, &ctx->drift_host[0], 4);
-        memcpy(&dh, &ctx->drift_host[1], 4);
-        ctx->drift_hist[0] = ctx->drift_hist[1];
-        ctx->drift_hist[1] = ctx->S_abs > 0.0 ? (2.0 * std::sqrt((double)d2) + ctx->radius_scale * (double)dh) / ctx->S_abs : 2.0;
-    }
+    ctx->drift_hist[0] = ctx->drift_hist[1];
+    ctx->drift_hist[1] = ctx->S_abs > 0.0 ? drift_need(ctx, ctx->drift_host) / ctx->S_abs : 2.0;
     if (!drift_within_skin(ctx, ctx->drift_host)) {
         // the evaluation that followed used stale lists: force the full rebuild
         build_invalid(ctx);
@@ -3620,84 +3618,28 @@ int b200sph_nnps_drift(b200sph_ctx *ctx, double out[2])
     if (retire_build(ctx)) return 0;
     if (ctx->n_sorted <= 0) { out[0] = 0.0; return 0; }
     if (!(ctx->packed_valid && ctx->drift_measured) && (rc = pack_positions_light(ctx, 2))) return rc;
+    ctx->packed_valid = true, ctx->drift_measured = true;
     CU(cudaMemcpyAsync(ctx->red_u32_host, ctx->red_u32, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
-    float d2, dh;
-    memcpy(&d2, &ctx->red_u32_host[0], 4);
-    memcpy(&dh, &ctx->red_u32_host[1], 4);
-    out[0] = 2.0 * std::sqrt((double)d2) + ctx->radius_scale * (double)dh;
+    out[0] = drift_need(ctx, ctx->red_u32_host);
     return 0;
-}
-
-int b200sph_halo_pack_selected_all(b200sph_ctx *ctx, int slot, double *dev_buf, int64_t cap_doubles, int64_t *ndoubles)
-{
-    CU(cudaSetDevice(ctx->device));
-    int rc = ensure_pool(ctx);
-    if (rc) return rc;
-    if ((rc = eos_flush(ctx))) return rc;
-    if (slot < 0 || slot > 1) return set_err(ctx, "halo_pack_selected_all: bad slot");
-    HaloAllArgs A;
-    A.narr = ctx->narr;
-    A.prefix[0] = 0;
-    for (int a = 0; a < ctx->narr; a++) {
-        A.prefix[a + 1] = A.prefix[a] + ctx->halo_cnt[a][slot];
-        A.off[a] = ctx->arr[a].off;
-        A.idx[a] = ctx->halo_idx[a][slot];
-    }
-    const int64_t tot = A.prefix[ctx->narr];
-    *ndoubles = tot * halo_nf(ctx);
-    if (*ndoubles > cap_doubles) return set_err(ctx, "halo_pack_selected_all: buffer too small");
-    if (tot == 0) return 0;
-    return with_halo_fields(ctx, [&](auto nf) {
-        k_halo_gather_all<decltype(nf)::value><<<(unsigned)cdiv(tot, 256), 256, 0, ctx->stream>>>(halo_ptrs(ctx), A, dev_buf);
-        LAUNCH_CHECK();
-        return 0;
-    });
 }
 
 // the ghost ranges [ghost_first[a], ghost_first[a] + counts[a]) of every array, checked against
 // the array's ghosts, as the scatter's HaloAllArgs
-static int ghost_ranges(b200sph_ctx *ctx, const char *who, const int64_t *ghost_first, const int64_t *counts, HaloAllArgs &A)
+static int ghost_ranges(b200sph_ctx *ctx, const int64_t *ghost_first, const int64_t *counts, HaloAllArgs &A)
 {
     A.narr = ctx->narr;
     A.prefix[0] = 0;
     for (int a = 0; a < ctx->narr; a++) {
         const ArrayInfo &ai = ctx->arr[a];
         if (ghost_first[a] < 0 || counts[a] < 0 || ai.n_real + ghost_first[a] + counts[a] > ai.n)
-            return set_err(ctx, "%s: ghosts [%lld, %lld) outside the %lld ghosts of '%s'", who, (long long)ghost_first[a],
+            return set_err(ctx, "peer_recv: ghosts [%lld, %lld) outside the %lld ghosts of '%s'", (long long)ghost_first[a],
                            (long long)(ghost_first[a] + counts[a]), (long long)(ai.n - ai.n_real), ai.name.c_str());
         A.prefix[a + 1] = A.prefix[a] + counts[a];
         A.off[a] = ai.off + ai.n_real + ghost_first[a];
         A.idx[a] = nullptr;
     }
-    return 0;
-}
-
-int b200sph_halo_overwrite_all(b200sph_ctx *ctx, const int64_t *ghost_first, const int64_t *counts, const double *dev_buf)
-{
-    CU(cudaSetDevice(ctx->device));
-    int rc = ensure_pool(ctx);
-    if (rc) return rc;
-    HaloAllArgs A;
-    if ((rc = ghost_ranges(ctx, "halo_overwrite_all", ghost_first, counts, A))) return rc;
-    const int64_t tot = A.prefix[ctx->narr];
-    if (tot == 0) return 0;
-    // with a reusable build whose packed positions are current (nnps_drift_device just
-    // ran) only the ghosts moved: refresh their packed records here and keep the flag
-    const bool repack = ctx->packed_valid && reusable_build(ctx) && ctx->n_sorted > 0;
-    RepackArgs R;
-    R.rank = repack ? ctx->rank : nullptr;
-    R.skey = ctx->skey;
-    R.A = ctx->A;
-    R.AB = ctx->AB;
-    R.G = ctx->G;
-    rc = with_halo_fields(ctx, [&](auto nf) {
-        k_halo_scatter_all<decltype(nf)::value><<<(unsigned)cdiv(tot, 256), 256, 0, ctx->stream>>>(halo_ptrs(ctx), A, dev_buf, R);
-        LAUNCH_CHECK();
-        return 0;
-    });
-    if (rc) return rc;
-    ghosts_refreshed(ctx, repack, false);
     return 0;
 }
 
@@ -3736,24 +3678,6 @@ int b200sph_ipc_close(b200sph_ctx *ctx, void *dev_ptr, int owner)
     CU(cudaStreamSynchronize(ctx->stream));
     if (owner) CU(cudaFree(dev_ptr));
     else CU(cudaIpcCloseMemHandle(dev_ptr));
-    return 0;
-}
-
-int b200sph_nnps_drift_device(b200sph_ctx *ctx, double *dev_ratio)
-{
-    CU(cudaSetDevice(ctx->device));
-    int rc = ensure_pool(ctx);
-    if (rc) return rc;
-    if (!reusable_build(ctx) || retire_build(ctx)) return 1;
-    if (ctx->n_sorted <= 0) {
-        CU(cudaMemsetAsync(dev_ratio, 0, sizeof(double), ctx->stream));
-        return 0;
-    }
-    if (!(ctx->packed_valid && ctx->drift_measured) && (rc = pack_positions_light(ctx, 2))) return rc;   // (the fused stage kernel packs and measures)
-    k_drift_ratio<<<1, 1, 0, ctx->stream>>>(ctx->red_u32, (float)ctx->radius_scale, (float)ctx->S_abs, dev_ratio);
-    LAUNCH_CHECK();
-    ctx->packed_valid = true;
-    ctx->drift_measured = true;
     return 0;
 }
 
@@ -3989,7 +3913,7 @@ int b200sph_peer_recv(b200sph_ctx *ctx, int side, const int64_t *ghost_first, co
     if (!ctx->peer_connected) return set_err(ctx, "peer_recv: the mailboxes are not connected");
     if (side < 0 || side > 1) return set_err(ctx, "peer_recv: bad side");
     HaloAllArgs A;
-    if (int rc = ghost_ranges(ctx, "peer_recv", ghost_first, counts, A)) return rc;
+    if (int rc = ghost_ranges(ctx, ghost_first, counts, A)) return rc;
     const int64_t tot = A.prefix[ctx->narr];
     if (tot == 0) return 0;
     int rc = refresh_ptype(ctx);

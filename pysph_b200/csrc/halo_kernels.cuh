@@ -116,64 +116,6 @@ __global__ void k_mirror_copy(HaloPtrs P, long long off, const uint32_t *__restr
         P.p[f][dst + k] = v;
     }
 }
-struct HaloAllArgs {
-    int narr;
-    long long prefix[B200SPH_MAX_ARRAYS + 1];  // particles before array a in the message
-    long long off[B200SPH_MAX_ARRAYS];         // pool offset of the first particle addressed
-    const uint32_t *idx[B200SPH_MAX_ARRAYS];   // gather: saved selection (relative to off); scatter: unused
-};
-// the refresh message of ALL arrays in one launch: block of array a starts at
-// NF * prefix[a] doubles, field-major and tight inside the block.  `dst` may be a peer
-// pointer (the neighbour's staging buffer): then this kernel is pack + send in one.
-template <int NF>
-__global__ void k_halo_gather_all(HaloPtrs P, HaloAllArgs A, double *__restrict__ dst)
-{
-    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= A.prefix[A.narr]) return;
-    int a = 0;
-    while (k >= A.prefix[a + 1]) a++;
-    const long long r = k - A.prefix[a], cnt = A.prefix[a + 1] - A.prefix[a];
-    const long long i = A.off[a] + A.idx[a][r];
-    double *out = dst + NF * A.prefix[a] + r;
-#pragma unroll
-    for (int f = 0; f < HALO_ND(NF); f++) out[(long long)f * cnt] = P.p[f][i];
-    if (NF != B200SPH_HALO_FIELDS) out[(long long)(NF - 1) * cnt] = (double)P.cs[i];
-}
-struct RepackArgs {
-    const uint32_t *rank, *skey;   // rank == nullptr: no repack
-    float4 *A, *AB;
-    GridDev G;
-};
-// ghost values refreshed in place; with a valid neighbour build the ghosts' packed
-// cell-relative positions are refreshed in the same pass (x, y, z, h are fields 0, 1, 2, 7)
-template <int NF>
-__global__ void k_halo_scatter_all(HaloPtrs P, HaloAllArgs A, const double *__restrict__ src, RepackArgs R)
-{
-    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= A.prefix[A.narr]) return;
-    int a = 0;
-    while (k >= A.prefix[a + 1]) a++;
-    const long long r = k - A.prefix[a], cnt = A.prefix[a + 1] - A.prefix[a];
-    const double *in = src + NF * A.prefix[a] + r;
-    double v[HALO_ND(NF)];
-#pragma unroll
-    for (int f = 0; f < HALO_ND(NF); f++) {
-        v[f] = in[(long long)f * cnt];
-        P.p[f][A.off[a] + r] = v[f];
-    }
-    if (NF != B200SPH_HALO_FIELDS) P.cs[A.off[a] + r] = (float)in[(long long)(NF - 1) * cnt];
-    if (R.rank) {
-        const uint32_t s = R.rank[A.off[a] + r];
-        const float4 q = pack_position(R.G, R.skey[s], v[0], v[1], v[2], v[7]);
-        R.A[s] = q;
-        R.AB[2 * s] = q;
-    }
-}
-__global__ void k_drift_ratio(const unsigned *__restrict__ red_u32, float kr, float S, double *__restrict__ out)
-{
-    const float need = 2.0f * sqrtf(__uint_as_float(red_u32[0])) + kr * __uint_as_float(red_u32[1]);
-    out[0] = S > 0.f ? (double)(need / S) : 2.0;
-}
 __global__ void k_save_idx(long long n, const uint32_t *__restrict__ flag, const uint32_t *__restrict__ pos,
                            uint32_t *__restrict__ idx)
 {
@@ -248,28 +190,44 @@ __device__ __forceinline__ bool peer_wait(const volatile unsigned long long *fla
     return true;
 }
 
-// lane r publishes this rank's scalars to rank r.  which = 0: refresh epoch (v0 = used-up
-// fraction of the neighbour-list skin, 2 = no reusable build; v1 = the dt proposal or +inf),
-// which = 1: the stand-alone time-step agreement (v1 = dt proposal).
+// the used-up fraction of the neighbour-list skin S: (2 |dx|max + k dh) / S from the drift
+// that k_pack_pos_light / the fused stage kernel max-reduced into red_u32[0..1] (|dx|^2 and
+// dh as fp32 bits); 2 (= expired) without a skin
+__device__ __forceinline__ double drift_ratio(const unsigned *__restrict__ red_u32, float kr, float S)
+{
+    const float need = 2.0f * sqrtf(__uint_as_float(red_u32[0])) + kr * __uint_as_float(red_u32[1]);
+    return S > 0.f ? (double)(need / S) : 2.0;
+}
+
+// this rank's scalars into the slot `sl` of one rank's mailbox: v0 = the drift ratio, 2 = no
+// reusable build (have_build 0), 0 = a rank without particles (have_build 2); v1 = the dt
+// proposal tc[2] (with_dt) or +inf
+__device__ __forceinline__ void peer_publish_slot(PeerSlot *sl, unsigned long long epoch, const unsigned *__restrict__ red_u32,
+                                                  float kr, float S, int have_build, const double *__restrict__ tc, int with_dt)
+{
+    double v0 = 2.0;                 // have_build == 0: no reusable build
+    if (have_build == 1) {
+        v0 = drift_ratio(red_u32, kr, S);
+    } else if (have_build == 2) {
+        v0 = 0.0;                    // a rank without particles keeps whatever the others keep
+    }
+    const double v1 = with_dt ? tc[2] : __longlong_as_double(0x7ff0000000000000LL);
+    sl->v[0] = v0;
+    sl->v[1] = v1;
+    __threadfence_system();
+    *(volatile unsigned long long *)&sl->seq = epoch;
+}
+
+// lane r publishes this rank's scalars to rank r.  which = 0: refresh epoch, which = 1: the
+// stand-alone time-step agreement (v1 = dt proposal).
 __global__ void k_peer_publish(PeerPtrs R, int rank, int world, unsigned long long epoch, int which,
                                const unsigned *__restrict__ red_u32, float kr, float S, int have_build,
                                const double *__restrict__ tc, int with_dt)
 {
     const int r = threadIdx.x;
     if (r >= world) return;
-    double v0 = 2.0;                 // have_build == 0: no reusable build
-    if (have_build == 1) {
-        const float need = 2.0f * sqrtf(__uint_as_float(red_u32[0])) + kr * __uint_as_float(red_u32[1]);
-        v0 = S > 0.f ? (double)(need / S) : 2.0;
-    } else if (have_build == 2) {
-        v0 = 0.0;                    // a rank without particles keeps whatever the others keep
-    }
-    const double v1 = with_dt ? tc[2] : __longlong_as_double(0x7ff0000000000000LL);
     PeerSlot *sl = which == 0 ? &R.box[r]->scal[epoch & 1][rank] : &R.box[r]->dts[epoch & 1][rank];
-    sl->v[0] = v0;
-    sl->v[1] = v1;
-    __threadfence_system();
-    *(volatile unsigned long long *)&sl->seq = epoch;
+    peer_publish_slot(sl, epoch, red_u32, kr, S, have_build, tc, with_dt);
 }
 
 // wait for every rank's scalars of this epoch: MAX of v0 -> decision (device + host),
@@ -305,79 +263,35 @@ __global__ void k_peer_reduce(PeerBox *mine, int world, unsigned long long epoch
     }
 }
 
-// One direction of the fused push / pull kernels below.
-struct PeerDir {
-    HaloAllArgs A;
-    double *buf;                 // push: the neighbour's staging buffer (peer pointer); pull: mine
-    unsigned long long *flag;    // push: data_seq in the neighbour's mailbox; pull: in mine
-    unsigned *done;              // push: block counter of this direction
-    unsigned nblocks;            // blocks of PEER_NT messages entries (0: the flag alone)
+// The refresh message of ALL arrays: the block of array a starts at NF * prefix[a] doubles,
+// field-major and tight inside the block.
+struct HaloAllArgs {
+    int narr;
+    long long prefix[B200SPH_MAX_ARRAYS + 1];  // particles before array a in the message
+    long long off[B200SPH_MAX_ARRAYS];         // pool offset of the first particle addressed
+    const uint32_t *idx[B200SPH_MAX_ARRAYS];   // gather: saved selection (relative to off); scatter: unused
 };
-#define PEER_NT 256
-struct PeerPushArgs {
-    PeerDir d[2];
-    int ndir;
-    // the scalars of k_peer_publish, sent by block 0
-    int rank, world, have_build, with_dt;
-    float kr, S;
-    const unsigned *red_u32;
-    const double *tc;
-};
-
-// The outgoing half of a refresh epoch in ONE launch: block 0 publishes this rank's scalars
-// to every mailbox (k_peer_publish's body) and raises the flag of a direction that has
-// nothing to carry; the other blocks are k_halo_gather_all into the neighbours' staging
-// buffers, and whichever block of a direction finishes last raises that neighbour's
-// data-ready flag (every block fences its stores first).
-template <int NF>
-__global__ void __launch_bounds__(PEER_NT) k_peer_push(HaloPtrs P, PeerPushArgs X, PeerPtrs R, unsigned long long epoch)
+// entry k (< prefix[narr]) of the message: array a, its r-th particle of cnt
+__device__ __forceinline__ int halo_entry(const HaloAllArgs &A, long long k, long long &r, long long &cnt)
 {
-    if (blockIdx.x == 0) {
-        const int r = threadIdx.x;
-        if (r < X.world) {
-            double v0 = 2.0;
-            if (X.have_build == 1) {
-                const float need = 2.0f * sqrtf(__uint_as_float(X.red_u32[0])) + X.kr * __uint_as_float(X.red_u32[1]);
-                v0 = X.S > 0.f ? (double)(need / X.S) : 2.0;
-            } else if (X.have_build == 2) {
-                v0 = 0.0;
-            }
-            const double v1 = X.with_dt ? X.tc[2] : __longlong_as_double(0x7ff0000000000000LL);
-            PeerSlot *sl = &R.box[r]->scal[epoch & 1][X.rank];
-            sl->v[0] = v0;
-            sl->v[1] = v1;
-            __threadfence_system();
-            *(volatile unsigned long long *)&sl->seq = epoch;
-        } else if (r >= 32 && r < 32 + X.ndir && X.d[r - 32].nblocks == 0) {
-            __threadfence_system();
-            *(volatile unsigned long long *)X.d[r - 32].flag = epoch;
-        }
-        return;
-    }
-    const unsigned b = blockIdx.x - 1;
-    const int d = b >= X.d[0].nblocks ? 1 : 0;
-    const PeerDir &D = X.d[d];
-    const long long k = (long long)(b - (d ? X.d[0].nblocks : 0u)) * PEER_NT + threadIdx.x;
-    if (k < D.A.prefix[D.A.narr]) {
-        int a = 0;
-        while (k >= D.A.prefix[a + 1]) a++;
-        const long long r = k - D.A.prefix[a], cnt = D.A.prefix[a + 1] - D.A.prefix[a];
-        const long long i = D.A.off[a] + D.A.idx[a][r];
-        double *out = D.buf + NF * D.A.prefix[a] + r;
+    int a = 0;
+    while (k >= A.prefix[a + 1]) a++;
+    r = k - A.prefix[a];
+    cnt = A.prefix[a + 1] - A.prefix[a];
+    return a;
+}
+// entry k gathered from the pool into the message at dst (a peer pointer: the neighbour's
+// staging buffer)
+template <int NF>
+__device__ __forceinline__ void halo_gather_entry(const HaloPtrs &P, const HaloAllArgs &A, long long k, double *__restrict__ dst)
+{
+    long long r, cnt;
+    const int a = halo_entry(A, k, r, cnt);
+    const long long i = A.off[a] + A.idx[a][r];
+    double *out = dst + NF * A.prefix[a] + r;
 #pragma unroll
-        for (int f = 0; f < HALO_ND(NF); f++) out[(long long)f * cnt] = P.p[f][i];
-        if (NF != B200SPH_HALO_FIELDS) out[(long long)(NF - 1) * cnt] = (double)P.cs[i];
-    }
-    __threadfence_system();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        const unsigned prev = atomicAdd(D.done, 1u);
-        if (prev == D.nblocks - 1) {
-            *D.done = 0;                     // re-armed for the next launch on this stream
-            __threadfence_system();
-            *(volatile unsigned long long *)D.flag = epoch;
-        }
-    }
+    for (int f = 0; f < HALO_ND(NF); f++) out[(long long)f * cnt] = P.p[f][i];
+    if (NF != B200SPH_HALO_FIELDS) out[(long long)(NF - 1) * cnt] = (double)P.cs[i];
 }
 
 // the packed pair records of a ghost, written by the receiving kernel (the fused stage
@@ -392,43 +306,21 @@ struct GhostPackArgs {
     int eos_any;
     EosTab E;
 };
-
-struct PeerPullArgs {
-    PeerDir d[2];
-    int ndir;
-};
-// The incoming half in ONE launch: k_halo_scatter_all of both neighbours' messages, every
-// block behind the data-ready flag of its own direction (a block of the left message does
-// not wait for the right neighbour).
+// entry k of the message at src (written by the peer: read past L1) scattered over its ghost
+// in place, and with a valid neighbour build the ghost's packed records refreshed in the
+// same pass (x, y, z, h are fields 0, 1, 2, 7)
 template <int NF>
-__global__ void __launch_bounds__(PEER_NT) k_peer_pull(HaloPtrs P, PeerPullArgs X, GhostPackArgs R, unsigned long long epoch,
-                                                       PeerDecision *dec_host)
+__device__ __forceinline__ void halo_scatter_entry(const HaloPtrs &P, const HaloAllArgs &A, long long k, const double *src,
+                                                   const GhostPackArgs &R)
 {
-    __shared__ int s_ok;
-    const int d = blockIdx.x >= X.d[0].nblocks ? 1 : 0;
-    const PeerDir &D = X.d[d];
-    const HaloAllArgs &A = D.A;
-    const double *src = D.buf;
-    if (threadIdx.x == 0) {
-        s_ok = peer_wait((const volatile unsigned long long *)D.flag, epoch) ? 1 : 0;
-        __threadfence_system();
-    }
-    __syncthreads();
-    if (!s_ok) {
-        if (threadIdx.x == 0 && dec_host) dec_host->error = epoch;
-        return;
-    }
-    const long long k = (long long)(blockIdx.x - (d ? X.d[0].nblocks : 0u)) * PEER_NT + threadIdx.x;
-    if (k >= A.prefix[A.narr]) return;
-    int a = 0;
-    while (k >= A.prefix[a + 1]) a++;
-    const long long r = k - A.prefix[a], cnt = A.prefix[a + 1] - A.prefix[a];
+    long long r, cnt;
+    const int a = halo_entry(A, k, r, cnt);
     const double *in = src + NF * A.prefix[a] + r;
     const long long g = A.off[a] + r;
     double v[HALO_ND(NF)];
 #pragma unroll
     for (int f = 0; f < HALO_ND(NF); f++) {
-        v[f] = __ldcg(in + (long long)f * cnt);      // written by the peer: not through L1
+        v[f] = __ldcg(in + (long long)f * cnt);
         P.p[f][g] = v[f];
     }
     if (NF != B200SPH_HALO_FIELDS) P.cs[g] = (float)__ldcg(in + (long long)(NF - 1) * cnt);
@@ -455,6 +347,88 @@ __global__ void __launch_bounds__(PEER_NT) k_peer_pull(HaloPtrs P, PeerPullArgs 
             R.C[s] = c;
         }
     }
+}
+
+// One direction of the fused push / pull kernels below.
+struct PeerDir {
+    HaloAllArgs A;
+    double *buf;                 // push: the neighbour's staging buffer (peer pointer); pull: mine
+    unsigned long long *flag;    // push: data_seq in the neighbour's mailbox; pull: in mine
+    unsigned *done;              // push: block counter of this direction
+    unsigned nblocks;            // blocks of PEER_NT messages entries (0: the flag alone)
+};
+#define PEER_NT 256
+struct PeerPushArgs {
+    PeerDir d[2];
+    int ndir;
+    // the scalars of k_peer_publish, sent by block 0
+    int rank, world, have_build, with_dt;
+    float kr, S;
+    const unsigned *red_u32;
+    const double *tc;
+};
+
+// The outgoing half of a refresh epoch in ONE launch: block 0 publishes this rank's scalars
+// to every mailbox and raises the flag of a direction that has nothing to carry; the other
+// blocks gather the messages into the neighbours' staging buffers, and whichever block of a
+// direction finishes last raises that neighbour's data-ready flag (every block fences its
+// stores first).
+template <int NF>
+__global__ void __launch_bounds__(PEER_NT) k_peer_push(HaloPtrs P, PeerPushArgs X, PeerPtrs R, unsigned long long epoch)
+{
+    if (blockIdx.x == 0) {
+        const int r = threadIdx.x;
+        if (r < X.world) {
+            peer_publish_slot(&R.box[r]->scal[epoch & 1][X.rank], epoch, X.red_u32, X.kr, X.S, X.have_build, X.tc, X.with_dt);
+        } else if (r >= 32 && r < 32 + X.ndir && X.d[r - 32].nblocks == 0) {
+            __threadfence_system();
+            *(volatile unsigned long long *)X.d[r - 32].flag = epoch;
+        }
+        return;
+    }
+    const unsigned b = blockIdx.x - 1;
+    const int d = b >= X.d[0].nblocks ? 1 : 0;
+    const PeerDir &D = X.d[d];
+    const long long k = (long long)(b - (d ? X.d[0].nblocks : 0u)) * PEER_NT + threadIdx.x;
+    if (k < D.A.prefix[D.A.narr]) halo_gather_entry<NF>(P, D.A, k, D.buf);
+    __threadfence_system();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const unsigned prev = atomicAdd(D.done, 1u);
+        if (prev == D.nblocks - 1) {
+            *D.done = 0;                     // re-armed for the next launch on this stream
+            __threadfence_system();
+            *(volatile unsigned long long *)D.flag = epoch;
+        }
+    }
+}
+
+struct PeerPullArgs {
+    PeerDir d[2];
+    int ndir;
+};
+// The incoming half in ONE launch: both neighbours' messages scattered over the ghosts, every
+// block behind the data-ready flag of its own direction (a block of the left message does
+// not wait for the right neighbour).
+template <int NF>
+__global__ void __launch_bounds__(PEER_NT) k_peer_pull(HaloPtrs P, PeerPullArgs X, GhostPackArgs R, unsigned long long epoch,
+                                                       PeerDecision *dec_host)
+{
+    __shared__ int s_ok;
+    const int d = blockIdx.x >= X.d[0].nblocks ? 1 : 0;
+    const PeerDir &D = X.d[d];
+    if (threadIdx.x == 0) {
+        s_ok = peer_wait((const volatile unsigned long long *)D.flag, epoch) ? 1 : 0;
+        __threadfence_system();
+    }
+    __syncthreads();
+    if (!s_ok) {
+        if (threadIdx.x == 0 && dec_host) dec_host->error = epoch;
+        return;
+    }
+    const long long k = (long long)(blockIdx.x - (d ? X.d[0].nblocks : 0u)) * PEER_NT + threadIdx.x;
+    if (k >= D.A.prefix[D.A.narr]) return;
+    halo_scatter_entry<NF>(P, D.A, k, D.buf, R);
 }
 
 // ---- interior / boundary split of the list consumer ---------------------------------------

@@ -9,10 +9,13 @@ Replaces the reference's Zoltan/MPI ``ParallelManager``
   solids 0.1, scheme.py:523-527);
 * ``update()`` (called from ``Integrator.compute_accelerations`` exactly like
   parallel_manager.pyx:512-530).  While every rank's neighbour lists are still
-  valid (one scalar all-reduce of the drift) only the VALUES of the same ghost
-  particles are refreshed: pack + send is one kernel per neighbour that writes
-  into the neighbour's cudaIpc staging buffer over NVLink (``_setup_peer``), the
-  all-reduce is the barrier, one kernel scatters.  Otherwise the full path runs:
+  valid (MAX of the drift over all ranks) only the VALUES of the same ghost
+  particles are refreshed.  On the ranks of one node that is the peer protocol
+  (include/b200sph.h, ``_setup_peer``): one kernel writes the messages into the
+  neighbours' cudaIpc staging buffers over NVLink and the drift into every
+  rank's mailbox, one kernel scatters, both under the interior pair work.
+  Without peer memory the messages go by send / recv behind one scalar
+  all-reduce of the drift.  Otherwise the full path runs:
   drop last build's Remote particles, migrate real particles that left the slab
   (all 16 fp64 state properties + gid, so that a mid-step migration keeps
   x0..rho0), import the neighbours' particles within one kernel support + skin of
@@ -104,8 +107,8 @@ class DeviceHaloOps(object):
         self.device = torch.device('cuda', device)
         # torch.distributed collectives and P2P only order against torch's current
         # stream; the library's own stream is a cudaStreamNonBlocking one.  Everything
-        # this class enqueues (drift_to, packs into peer staging, appends that read
-        # receive buffers, the dt block NCCL reduces in place) must therefore run on
+        # this class enqueues (packs that NCCL sends, appends that read receive
+        # buffers, the dt block NCCL reduces in place) must therefore run on
         # torch's stream -- adopt it here instead of trusting the caller to.
         # (no CUDA in the process = the host emulation of the library used by the CPU
         # tests, where streams are no-ops; a real backend cannot exist without a device)
@@ -191,21 +194,7 @@ class DeviceHaloOps(object):
             return float(self._pin[0])
         return get
 
-    # -- all arrays in one kernel; peer (NVLink) staging ------------------------
-    def pack_selected_all(self, slot, ptr, cap_doubles):
-        """Refresh message of every array for neighbour `slot`, written to the
-        raw device pointer `ptr` -- a local buffer or a neighbour's staging
-        buffer mapped with ipc_open (then pack and send are one kernel)."""
-        nd = C.c_int64()
-        self.ctx.call('b200sph_halo_pack_selected_all', slot, ptr, int(cap_doubles),
-                      C.byref(nd))
-        return nd.value
-
-    def overwrite_all(self, ghost_first, counts, ptr):
-        n = self.narr
-        self.ctx.call('b200sph_halo_overwrite_all', (C.c_int64 * n)(*ghost_first),
-                      (C.c_int64 * n)(*counts), ptr)
-
+    # -- peer (NVLink) staging buffers ---------------------------------------------
     def ipc_alloc(self, nbytes):
         ptr = C.c_void_p()
         handle = C.create_string_buffer(64)
@@ -267,13 +256,6 @@ class DeviceHaloOps(object):
 
     def peer_allreduce_dt(self):
         self.ctx.call('b200sph_peer_allreduce_dt')
-
-    def drift_to(self, tensor):
-        """Write the used-up fraction of the skin into a 1-element CUDA double
-        tensor (no host sync); 2.0 if there is no reusable build."""
-        rc = self.ctx.call('b200sph_nnps_drift_device', tensor.data_ptr())
-        if rc == 1:
-            tensor.fill_(2.0)
 
     def drift(self):
         """(need, skin): the neighbour build is reusable while need <= skin;
@@ -344,16 +326,14 @@ class SlabParallelManager(object):
         # last full exchange (the refresh path re-sends exactly those particles)
         self._sent = {}
         self._recv = {}
-        # peer-memory refresh (GPUs of one node): per neighbour two staging buffers
-        # (double buffered by evaluation parity) that the NEIGHBOUR writes into
+        # peer protocol (GPUs of one node): per neighbour two staging buffers (double
+        # buffered by evaluation parity) that the NEIGHBOUR writes into, the scalar
+        # agreements through mailboxes in peer memory, the refresh on a second stream
+        # under the interior pair work.  B200SPH_PEER_HALO=0: send / recv instead
         self.use_peer = bool(int(__import__('os').environ.get('B200SPH_PEER_HALO', '1'))) \
             and hasattr(ops, 'ipc_alloc')
-        self._peer = None
+        self._peer = None             # the staging buffers, set with _peer_sync
         self._parity = 0
-        # peer protocol: the scalar agreements go through mailboxes in peer memory too and
-        # the refresh runs on a second stream under the interior pair work
-        self.use_peer_sync = self.use_peer and hasattr(ops, 'peer_begin') and \
-            bool(int(__import__('os').environ.get('B200SPH_PEER_SYNC', '1')))
         self._peer_sync = False
         self._dt_pending = None       # (prev, new, adaptive, advance, slot): agreement + commit deferred
         # proactive full update: the global used-up fraction of the skin at the last two
@@ -479,7 +459,7 @@ class SlabParallelManager(object):
         self.lb_count += 1
         if self._prof is not None:
             self._prof['n'] += 1
-        if self._recv and self._peer is not None and self._peer_sync:
+        if self._recv and self._peer_sync:
             r0, r1 = self._ratio_hist
             if deferred and self.proactive and r1 >= 0.0 and \
                     r1 + (max(r1 - r0, 0.0) if r0 >= 0.0 else r1) > 0.9:
@@ -498,24 +478,9 @@ class SlabParallelManager(object):
                 self._t1 = ops.new_buffer(1)
             t = self._t1
             self._ev()
-            if hasattr(ops, 'drift_to'):
-                ops.drift_to(t)           # stays on the device until the all-reduce
-            else:
-                need, skin = ops.drift()
-                t.fill_(need / skin if (need >= 0.0 and skin > 0.0) else 2.0)
-            if self._peer is not None:
-                # speculative pack + send in ONE kernel per neighbour: the values go
-                # straight into the neighbour's staging buffer over NVLink; the
-                # all-reduce below is both the decision and the barrier that makes
-                # them visible (double buffering keeps the previous evaluation's
-                # buffer untouched while a slower neighbour may still read it)
-                self._parity ^= 1
-                for nb in self._peer['nbs']:
-                    slot = 0 if nb == self.left else 1
-                    if sum(self._sent[nb]):
-                        ops.pack_selected_all(slot, self._peer['remote'][nb][self._parity],
-                                              self._peer['cap'])
-            self._ev('drift+send')
+            need, skin = ops.drift()
+            t.fill_(need / skin if (need >= 0.0 and skin > 0.0) else 2.0)
+            self._ev('drift')
             t_ar = time.perf_counter()
             self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX)
             self._cpu('all_reduce_call', t_ar)
@@ -526,16 +491,7 @@ class SlabParallelManager(object):
             else:
                 ok = float(t.item()) <= 0.9
             if ok:
-                if self._peer is not None:
-                    first = [0] * self.narr
-                    for nb in sorted(self._recv):
-                        if sum(self._recv[nb]):
-                            ops.overwrite_all(first, self._recv[nb],
-                                              self._peer['local'][nb][self._parity])
-                        first = [f + n for f, n in zip(first, self._recv[nb])]
-                    self.n_peer_refresh += 1
-                else:
-                    self._refresh_ghosts()
+                self._refresh_ghosts()
                 self._ev('overwrite')
                 if hasattr(ops, 'keep_build'):
                     if not ops.keep_build(strict=self._pending is None):
@@ -674,7 +630,10 @@ class SlabParallelManager(object):
 
     def _setup_peer(self):
         """(Re)allocate the staging buffers when the halo outgrew them and exchange
-        their IPC handles with the slab neighbours.  Collective; full path only."""
+        their IPC handles with the slab neighbours; the first time also map every
+        rank's mailbox.  Collective; full path only.  If any rank fails any step,
+        every rank releases the staging buffers it allocated or mapped and refreshes
+        by send / recv from then on."""
         ops, dist = self.ops, self.dist
         nbs = [nb for nb in (self.left, self.right) if nb is not None]
         need = max([sum(self._recv[nb]) for nb in nbs] +
@@ -685,80 +644,64 @@ class SlabParallelManager(object):
         need = int(t.item())
         if self._peer is not None and need <= self._peer['cap']:
             return
-        def all_ok(flag):
-            t.fill_(1.0 if flag else 0.0)
-            dist.all_reduce(t, op=dist.ReduceOp.MIN)
-            return float(t.item()) > 0.5
 
         def warn(e):
             import sys
-            sys.stderr.write('pysph_b200: peer-memory halo disabled (%s)\n' % e)
+            sys.stderr.write('pysph_b200: peer protocol disabled (%s)\n' % e)
 
-        if self._peer is not None:      # retire the old buffers (collectively)
-            for nb in self._peer['nbs']:
-                for p in self._peer['remote'][nb]:
-                    ops.ipc_close(p, False)
-            dist.barrier()              # nobody still maps a buffer that is freed next
-            for nb in self._peer['nbs']:
-                for p in self._peer['local'][nb]:
-                    ops.ipc_close(p, True)
+        if self._peer is not None:
+            self._release_peer(self._peer)
             self._peer = None
         cap = int(need * 1.5) + 1024
-        local, handles, ok = {}, {}, True
+        peer = dict(nbs=nbs, cap=cap, local=dict((nb, []) for nb in nbs),
+                    remote=dict((nb, []) for nb in nbs))
+        handles = dict((nb, []) for nb in nbs)
+        mailbox, ok = None, True
         try:
             for nb in nbs:
-                bufs = [ops.ipc_alloc(8 * cap) for _ in range(2)]
-                local[nb] = [b_[0] for b_ in bufs]
-                handles[nb] = [b_[1] for b_ in bufs]
+                for _ in range(2):
+                    ptr, h = ops.ipc_alloc(8 * cap)
+                    peer['local'][nb].append(ptr)
+                    handles[nb].append(h)
+            if not self._peer_sync:
+                mailbox = ops.peer_init(self.rank, self.world)
         except Exception as e:          # e.g. IPC not permitted in this container
             warn(e)
             ok = False
-        if not all_ok(ok):
-            self.use_peer = False
-            return
         gathered = [None] * self.world
-        dist.all_gather_object(gathered, handles)
-        remote = {}
-        try:
-            # the buffer I write into on neighbour nb is the one nb allocated for ME
-            for nb in nbs:
-                remote[nb] = [ops.ipc_open(h) for h in gathered[nb][self.rank]]
-        except Exception as e:
-            warn(e)
-            ok = False
-        if not all_ok(ok):
-            self.use_peer = False
-            return
-        self._peer = dict(nbs=nbs, cap=cap, local=local, remote=remote)
-        self._setup_peer_sync()
-
-    def _setup_peer_sync(self):
-        """Once: every rank maps every rank's mailbox (collective)."""
-        if not self.use_peer_sync or self._peer_sync:
-            return
-        ops, dist = self.ops, self.dist
-        ok, handle = True, None
-        try:
-            handle = ops.peer_init(self.rank, self.world)
-        except Exception as e:
-            __import__('sys').stderr.write('pysph_b200: peer protocol disabled (%s)\n' % e)
-            ok = False
-        gathered = [None] * self.world
-        dist.all_gather_object(gathered, handle)
-        ok = ok and all(h is not None for h in gathered)
-        if ok:
+        dist.all_gather_object(gathered, (handles, mailbox) if ok else None)
+        if all(g is not None for g in gathered):
             try:
-                ops.peer_connect(gathered)
+                # the buffer I write into on neighbour nb is the one nb allocated for ME
+                for nb in nbs:
+                    for h in gathered[nb][0][self.rank]:
+                        peer['remote'][nb].append(ops.ipc_open(h))
+                if not self._peer_sync:
+                    ops.peer_connect([g[1] for g in gathered])
             except Exception as e:
-                __import__('sys').stderr.write('pysph_b200: peer protocol disabled (%s)\n' % e)
+                warn(e)
                 ok = False
-        t = ops.new_buffer(1)
+        else:
+            ok = False
         t.fill_(1.0 if ok else 0.0)
         dist.all_reduce(t, op=dist.ReduceOp.MIN)
         if float(t.item()) > 0.5:
+            self._peer = peer
             self._peer_sync = True
         else:
-            self.use_peer_sync = False
+            self._release_peer(peer)
+            self.use_peer = False
+            self._peer_sync = False
+
+    def _release_peer(self, peer):
+        """Unmap the neighbours' staging buffers, then free my own.  Collective."""
+        for nb in peer['nbs']:
+            for p in peer['remote'][nb]:
+                self.ops.ipc_close(p, False)
+        self.dist.barrier()             # nobody still maps a buffer that is freed next
+        for nb in peer['nbs']:
+            for p in peer['local'][nb]:
+                self.ops.ipc_close(p, True)
 
     def _refresh_ghosts(self):
         ops = self.ops

@@ -13,6 +13,7 @@ pytestmark = pytest.mark.gpu
 
 DX = 0.04
 NSTEPS = 25
+F9 = ['x', 'y', 'z', 'u', 'v', 'w', 'rho', 'h', 'm']        # the ghost message
 
 
 def _ngpus():
@@ -51,6 +52,44 @@ def _collect(pas):
     return out
 
 
+def _refreshed_ghosts(solver, pm, pas, fields):
+    """After the steps: pm.update() until the ghosts have been refreshed in place (a full
+    update on the way is followed by the sort and the evaluation that build the lists a
+    refresh needs), then every array's real particles and ghosts, the fields of the ghost
+    message as the host sees them."""
+    n0 = pm.n_refresh
+    for _ in range(4):
+        pm.update()
+        if pm.n_refresh > n0:
+            break
+        solver.nnps.update()
+        solver.integrator.compute_accelerations(update_nnps=False)
+    solver.pull()
+    out = {}
+    for pa in pas:
+        nr = pa.get_number_of_particles(real=True)
+        out[pa.name] = (dict((k, pa.properties[k][:nr].copy()) for k in fields),
+                        dict((k, pa.properties[k][nr:].copy()) for k in fields))
+    return out, pm.n_refresh - n0, pm.n_peer_refresh
+
+
+def _assert_ghosts_are_their_owners(per_rank, fields):
+    """Every rank's ghosts matched to their owner among all ranks' real particles by the
+    exact (x, y, z): every field of the ghost message is bitwise the owner's."""
+    nghost = 0
+    for name in per_rank[0]:
+        real = dict((k, np.concatenate([o[name][0][k] for o in per_rank])) for k in fields)
+        owner = dict((p, i) for i, p in enumerate(zip(real['x'], real['y'], real['z'])))
+        assert len(owner) == real['x'].size, name
+        for o in per_rank:
+            g = o[name][1]
+            idx = np.array([owner[p] for p in zip(g['x'], g['y'], g['z'])], dtype=np.int64)
+            for k in fields:
+                assert np.array_equal(g[k].view(np.uint64), real[k][idx].view(np.uint64)), (name, k)
+            nghost += idx.size
+    assert nghost > 0
+
+
 def _worker(rank, world, port, q):
     import torch
     import torch.distributed as dist
@@ -73,8 +112,9 @@ def _worker(rank, world, port, q):
         for _ in range(NSTEPS):
             solver.step()
         solver.pull()
-        q.put((rank, _collect(pas), pm.n_full, pm.n_refresh,
-               solver.backend.stats(), pm.n_peer_refresh))
+        res = (rank, _collect(pas), pm.n_full, pm.n_refresh, solver.backend.stats(),
+               pm.n_peer_refresh)
+        q.put(res + _refreshed_ghosts(solver, pm, pas, F9))
     finally:
         dist.destroy_process_group()
 
@@ -114,6 +154,9 @@ def test_slab_decomposition_matches_single_gpu(world):
     assert min(n_refresh) > 0 and min(n_full) >= 2, (n_full, n_refresh)
     # the refreshes went over peer memory (NVLink stores), not NCCL send/recv
     assert min(o[5] for o in out) > 0, [o[5] for o in out]
+    # one more refresh on the peer protocol: every ghost carries its owner's current values
+    assert all(o[7] > 0 and o[8] > o[5] for o in out), [(o[7], o[8], o[5]) for o in out]
+    _assert_ghosts_are_their_owners([o[6] for o in out], F9)
     h0, c0 = params['h0'], params['c0']
     for name in ref:
         g_all = np.concatenate([o[1][name]['gid'] for o in out])

@@ -9,8 +9,9 @@ import os
 import numpy as np
 import pytest
 
-from test_gpu_multi import _free_port, _ngpus
-from test_library_on_cpu import RINGS, RING_FIELDS, _rings_collect, _rings_perturb
+from test_gpu_multi import (F9, _assert_ghosts_are_their_owners, _free_port, _ngpus,
+                            _refreshed_ghosts)
+from test_library_on_cpu import RINGS, RING_FIELDS, RING_MESSAGE, _rings_collect, _rings_perturb
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(300)]
 
@@ -34,7 +35,8 @@ def _worker(rank, world, port, q):
         for _ in range(RINGS['steps']):
             solver.step()
         solver.pull()
-        q.put((rank, _rings_collect(pas[0]), pm.n_full, pm.n_refresh, pm.n_peer_refresh))
+        res = (rank, _rings_collect(pas[0]), pm.n_full, pm.n_refresh, pm.n_peer_refresh)
+        q.put(res + _refreshed_ghosts(solver, pm, pas, RING_MESSAGE))
     finally:
         dist.destroy_process_group()
 
@@ -64,6 +66,10 @@ def test_rings_slabs_match_single_gpu():
         p.join(timeout=60)
         assert p.exitcode == 0
     assert min(o[2] for o in out) >= 2
+    # one more refresh on the peer protocol: every ghost carries its owner's current values,
+    # the deviatoric stress and cs (fp32) included
+    assert all(o[6] > 0 and o[7] > o[4] for o in out), [(o[6], o[7], o[4]) for o in out]
+    _assert_ghosts_are_their_owners([o[5] for o in out], RING_MESSAGE)
     g_all = np.concatenate([o[1]['gid'] for o in out])
     assert np.array_equal(np.sort(g_all), np.sort(ref['gid']))
     order_ref, order = np.argsort(ref['gid']), np.argsort(g_all)
@@ -77,7 +83,6 @@ def test_rings_slabs_match_single_gpu():
 
 
 S6 = ['s00', 's01', 's02', 's11', 's12', 's22']
-F9 = ['x', 'y', 'z', 'u', 'v', 'w', 'rho', 'h', 'm']
 F16 = F9 + ['x0', 'y0', 'z0', 'u0', 'v0', 'w0', 'rho0']
 
 
@@ -120,25 +125,6 @@ def test_elastic_halo_and_migration_layout(gpu_device):
         assert np.array_equal(b.properties[k][n:], ref[k][sel]), k
     assert np.array_equal(b.cs[n:], cs32[sel]) and np.all(b.s000[n:] == 0.0)
     assert np.all(b.tag[n:] == 1)
-    # the refresh message of ALL arrays in one kernel (what the peer-memory path sends) and
-    # its scatter onto the existing ghosts: same layout, current values
-    a.s01[:] = ref['s01'] + 3.0
-    a.cs[:] = ref['cs'] * 2.0
-    be.push(0, ['s01', 'cs'])
-    buf2 = ops.new_buffer(16 * n)
-    nd = ops.pack_selected_all(1, buf2.data_ptr(), buf2.numel())
-    assert nd == 16 * cnt
-    got2 = buf2[:nd].cpu().numpy().reshape(16, cnt)
-    assert np.array_equal(got2[10], ref['s01'][sel] + 3.0) and np.array_equal(got2[0], ref['x'][sel])
-    assert np.array_equal(got2[15], (ref['cs'] * 2.0).astype(np.float32).astype(np.float64)[sel])
-    ops.overwrite_all([0, 0], [0, cnt], buf2.data_ptr())
-    be.pull(1, ['s01', 'cs', 'x'])
-    assert np.array_equal(b.s01[n:], ref['s01'][sel] + 3.0)
-    assert np.array_equal(b.cs[n:], (ref['cs'] * 2.0).astype(np.float32).astype(np.float64)[sel])
-    assert np.array_equal(b.x[n:], ref['x'][sel])
-    a.s01[:] = ref['s01']
-    a.cs[:] = ref['cs']
-    be.push(0, ['s01', 'cs'])
     ops.drop_ghosts(1)
     mbuf = ops.new_buffer(30 * n)
     n_lo, n_hi = ops.migrate_out(0, 0.5, 2.5, mbuf, 0)

@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), 'libb200sph.so does not export %s' % name
     # and the ctypes table covers exactly the header
     assert set(_lib.SIGNATURES) == declared
-    assert lib.b200sph_abi_version() == 5
+    assert lib.b200sph_abi_version() == 6
 
 
 def test_no_cpu_fallback_without_device():

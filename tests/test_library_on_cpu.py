@@ -92,7 +92,7 @@ def test_every_entry_point_is_exported(emulated_library):
     lib = _lib.load()
     for name in _lib.SIGNATURES:
         assert hasattr(lib, name), name
-    assert lib.b200sph_abi_version() == 5
+    assert lib.b200sph_abi_version() == 6
 
 
 # ---- the GPU tests of this repository, run against the emulated library --------------------
@@ -516,8 +516,9 @@ def _slab_worker(rank, world, port, so, q, lb_freq=0):
             solver.step()
         t, dt = solver.t, solver.dt
         solver.pull()
-        q.put((rank, M._collect(pas), pm.n_full, pm.n_refresh, pm.n_deferred_failed, t, dt,
-               pm.use_peer, pm.n_recut, list(pm.cuts), pm.n_peer_refresh))
+        res = (rank, M._collect(pas), pm.n_full, pm.n_refresh, pm.n_deferred_failed, t, dt,
+               pm.use_peer, pm.n_recut, list(pm.cuts), pm.n_peer_refresh, pm._peer_sync)
+        q.put(res + M._refreshed_ghosts(solver, pm, pas, M.F9))
     except Exception:
         import traceback
         q.put(('error', rank, traceback.format_exc()))
@@ -565,11 +566,14 @@ def test_slab_decomposition_on_the_emulated_library(emulated_library, world, lb_
         assert p.exitcode == 0
     assert min(o[3] for o in out) > 0 and min(o[2] for o in out) >= 1      # refreshes and full paths
     if lb_freq:         # refresh through send / recv (B200SPH_PEER_HALO=0)
-        assert not any(o[7] for o in out) and not any(o[10] for o in out)
-    elif any(o[7] for o in out):   # refresh through the neighbours' staging buffers ("NVLink stores")
-        assert all(o[7] for o in out) and min(o[10] for o in out) > 0
+        assert not any(o[7] or o[10] or o[11] for o in out)
+    elif any(o[7] for o in out):   # refresh on the peer protocol ("NVLink stores" + mailboxes)
+        assert all(o[7] and o[11] for o in out) and min(o[10] for o in out) > 0
     else:               # shared mappings unavailable in this sandbox: the manager fell back, collectively
-        assert not any(o[10] for o in out)
+        assert not any(o[10] or o[11] for o in out)
+    # one more refresh on the same path: every ghost carries its owner's current values
+    assert all(o[13] > 0 and (o[14] > o[10]) == o[11] for o in out), [o[13:] for o in out]
+    M._assert_ghosts_are_their_owners([o[12] for o in out], M.F9)
     if lb_freq:         # the slabs were re-cut on the way (k_column_counts + migration)
         static = parallel.balanced_cuts(*parallel.dam_break_column_weights(
             SLAB_DX, solid_weight=0.45), world, SLAB_DX)
@@ -608,6 +612,9 @@ def test_halo_entry_points_on_the_emulated_library(emulated_library, monkeypatch
 
 RINGS = dict(dx=0.0025, lz=0.0075, dt=2e-7, steps=10, u_f=0.25)
 RING_FIELDS = ('x', 'y', 'z', 'u', 'v', 'w', 'rho', 's00', 's01', 's02', 's11', 's12', 's22')
+# the ghost message with the elastic-dynamics arrays
+RING_MESSAGE = ['x', 'y', 'z', 'u', 'v', 'w', 'rho', 'h', 'm', 's00', 's01', 's02', 's11', 's12',
+                's22', 'cs']
 
 
 def _rings_perturb(pa):
@@ -629,6 +636,7 @@ def _rings_worker(rank, world, port, so, q):
     from pysph_b200 import _lib
     _lib.LIB_PATH, _lib._lib = so, None
     from pysph_b200 import parallel
+    import test_gpu_multi as M
 
     Base = parallel.DeviceHaloOps
 
@@ -655,8 +663,10 @@ def _rings_worker(rank, world, port, so, q):
         for _ in range(RINGS['steps']):
             solver.step()
         solver.pull()
-        q.put((rank, _rings_collect(pas[0]), pm.n_full, pm.n_refresh, n0,
-               pas[0].get_number_of_particles(real=True), pm.use_peer, pm.n_peer_refresh))
+        res = (rank, _rings_collect(pas[0]), pm.n_full, pm.n_refresh, n0,
+               pas[0].get_number_of_particles(real=True), pm.use_peer, pm.n_peer_refresh,
+               pm._peer_sync)
+        q.put(res + M._refreshed_ghosts(solver, pm, pas, RING_MESSAGE))
     except Exception:
         import traceback
         q.put(('error', rank, traceback.format_exc()))
@@ -675,6 +685,7 @@ def test_rings_slab_decomposition_on_the_emulated_library(emulated_library):
     import torch.multiprocessing as mp
     import pysph_b200 as pb
     from pysph_b200 import geometry as geo, _lib
+    import test_gpu_multi as M
     world = 3
     pa = geo.rings_3d_particles(dx=RINGS['dx'], lz=RINGS['lz'], u_f=RINGS['u_f'])
     _rings_perturb(pa)
@@ -702,10 +713,17 @@ def test_rings_slab_decomposition_on_the_emulated_library(emulated_library):
         assert p.exitcode == 0
     assert min(o[2] for o in out) >= 2                  # full paths (rebuild + migration)
     assert any(o[4] != o[5] for o in out)               # somebody gained / lost particles
-    # refreshes went through the neighbours' staging buffers (k_halo_gather_all / scatter_all<16>)
+    # refreshes went through the peer protocol (k_peer_push / k_peer_pull<16>)
     # (if shared mappings are unavailable in this sandbox the manager falls back, collectively)
     if any(o[6] for o in out):
-        assert all(o[6] for o in out) and min(o[7] for o in out) > 0, [(o[6], o[7]) for o in out]
+        assert all(o[6] and o[8] for o in out) and min(o[7] for o in out) > 0, \
+            [(o[6], o[7], o[8]) for o in out]
+    else:
+        assert not any(o[7] or o[8] for o in out)
+    # one more refresh on the same path: every ghost carries its owner's current values, the
+    # deviatoric stress and cs (fp32) included
+    assert all(o[10] > 0 and (o[11] > o[7]) == o[8] for o in out), [o[10:] for o in out]
+    M._assert_ghosts_are_their_owners([o[9] for o in out], RING_MESSAGE)
     g_all = np.concatenate([o[1]['gid'] for o in out])
     assert np.array_equal(np.sort(g_all), np.sort(ref['gid']))
     order_ref, order = np.argsort(ref['gid']), np.argsort(g_all)
