@@ -66,9 +66,7 @@ enum {
     /* elastic-dynamics extension (solid_mech/basic.py:52-59), device memory allocated
      * on first use.  Symmetric tensors as 00 01 02 11 12 22, the velocity gradient as
      * 00 01 02 10 11 12 20 21 22.  fp64: deviatoric stress (integrated) and its copy;
-     * fp32: velocity gradient, artificial stress, stress rate.
-     * NOTE: written after this round's GPU budget was spent -- compiled, not yet run on
-     * hardware (tests/test_zz_gpu_solid_unvalidated.py) */
+     * fp32: velocity gradient, artificial stress, stress rate. */
     B200SPH_S00 = 70, B200SPH_S01, B200SPH_S02, B200SPH_S11, B200SPH_S12, B200SPH_S22,
     B200SPH_S000 = 76, B200SPH_S010, B200SPH_S020, B200SPH_S110, B200SPH_S120, B200SPH_S220,
     B200SPH_V00 = 82, B200SPH_V01, B200SPH_V02, B200SPH_V10, B200SPH_V11, B200SPH_V12,

@@ -36,6 +36,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <iterator>
 #include <string>
 #include <memory>
 #include <mutex>
@@ -45,11 +46,7 @@
 // --------------------------------------------------------------------------
 // small helpers
 // --------------------------------------------------------------------------
-#define N_F64 16
-#define N_F32 11
-#define N_U32 3
-#define N_F64X 5   // UHAT VHAT WHAT PF PF0 (ids 27..31)
-#define N_F32X 6   // VOL PAVG AUHAT AVHAT AWHAT AP (ids 32..37)
+#define N_PROP_SLOTS (B200SPH_USER0 + B200SPH_MAX_USER)   // property ids 0 .. the last user property
 #define PT_INVALID 0xFFu
 #define PT_GHOST 0x08u
 
@@ -238,20 +235,13 @@ struct b200sph_ctx {
     ArrayInfo arr[B200SPH_MAX_ARRAYS];
     int64_t pool_cap = 0;   // allocated particles in the pool
     int64_t pool_end = 0;   // off[last] + cap[last]
-    // by property id.  Which buffer goes by x .. rho and which by x0 .. rho0 changes when a fused
-    // stage 1 takes the initialize by renaming (init_by_rename): read these at enqueue time, and
-    // keep no copy of them across a stage
-    double *f64[N_F64] = {nullptr};
-    float *f32[N_F32] = {nullptr};
-    uint32_t *u32[N_U32] = {nullptr};
-    double *f64x[N_F64X] = {nullptr};   // transport-velocity / EDAC extension
-    float *f32x[N_F32X] = {nullptr};
+    // the property buffers by property id (prop_kind: element type and when it is allocated; null
+    // until then, and for ids the header does not define).  Which buffer goes by x .. rho and
+    // which by x0 .. rho0 changes when a fused stage 1 takes the initialize by renaming
+    // (init_by_rename): read these at enqueue time, and keep no copy of them across a stage
+    void *prop[N_PROP_SLOTS] = {nullptr};
     float4 *Dv = nullptr;               // sorted: (uhat-u, vhat-v, what-w, pavg)
-    // elastic-dynamics extension, allocated on first use (ensure_solid)
-    bool solid_alloc = false;
-    double *f64s[12] = {nullptr};       // s00 s01 s02 s11 s12 s22, then their *0 copies
-    float *f32s[21] = {nullptr};        // v00..v22 (9), r00..r22 (6), as00..as22 (6)
-    float4 *T01 = nullptr, *T2R = nullptr, *R2 = nullptr;   // sorted stress records
+    float4 *T01 = nullptr, *T2R = nullptr, *R2 = nullptr;   // sorted stress records (with the elastic group)
     float2 *PT = nullptr;               // sorted: (p, type)
     uint8_t *ptype = nullptr;
     bool ptype_dirty = true;
@@ -396,8 +386,7 @@ struct b200sph_ctx {
     // The scalar agreement runs on its own stream: a rank's ghosts only need its two neighbours,
     // the decision needs every rank, and the boundary launch must not wait for the slowest one.
     cudaStream_t red_stream = nullptr;
-    // generic-equation fallback: user properties (fp64, pool-wide) and run-time compiled modules
-    double *user_f64[B200SPH_MAX_USER] = {nullptr};
+    // generic-equation fallback: run-time compiled modules
     std::vector<void *> gen_modules;             // CUmodule (or, emulated, a dlopen handle)
     // density_filter: its records, [2 n_sorted] (allocated on first use)
     float4 *dfilter_F = nullptr;
@@ -663,38 +652,33 @@ __device__ __forceinline__ void rec32_make(const float4 A, const double u, const
 // --------------------------------------------------------------------------
 // host side
 // --------------------------------------------------------------------------
-static int is_solid_prop(int p) { return p >= B200SPH_S00 && p < B200SPH_SOLID_PROPS_END; }
-static int is_user_prop(int p) { return p >= B200SPH_USER0 && p < B200SPH_USER0 + B200SPH_MAX_USER; }
-static int is_f64_prop(int p)
+// What a property id of the header's enum is: its element type on the device (PROP_NONE: no such
+// property) and when its buffer is allocated -- with the pool, as a group the first time any
+// elastic-dynamics property is named (with the stress records T01 T2R R2), or one by one when a
+// user property is named.  The only host code that knows the ranges of the id enum.
+enum PropType { PROP_NONE, PROP_F64, PROP_F32, PROP_U32 };
+enum PropGroup { GROUP_POOL, GROUP_ELASTIC, GROUP_USER };
+struct PropKind {
+    PropType type;
+    PropGroup group;
+    size_t size() const { return type == PROP_F64 ? 8 : 4; }
+};
+static PropKind prop_kind(int p)
 {
-    return (p >= 0 && p < N_F64) || (p >= B200SPH_UHAT && p <= B200SPH_PF0) || (p >= B200SPH_S00 && p <= B200SPH_S220) ||
-           is_user_prop(p);
+    if (p >= B200SPH_X && p <= B200SPH_RHO0) return {PROP_F64, GROUP_POOL};
+    if (p >= B200SPH_P && p <= B200SPH_DT_FORCE) return {PROP_F32, GROUP_POOL};
+    if (p >= B200SPH_UHAT && p <= B200SPH_PF0) return {PROP_F64, GROUP_POOL};
+    if (p >= B200SPH_VOL && p <= B200SPH_AP) return {PROP_F32, GROUP_POOL};
+    if (p >= B200SPH_GID && p <= B200SPH_PID) return {PROP_U32, GROUP_POOL};
+    if (p >= B200SPH_S00 && p <= B200SPH_S220) return {PROP_F64, GROUP_ELASTIC};
+    if (p >= B200SPH_V00 && p <= B200SPH_AS22) return {PROP_F32, GROUP_ELASTIC};
+    if (p >= B200SPH_USER0 && p < B200SPH_USER0 + B200SPH_MAX_USER) return {PROP_F64, GROUP_USER};
+    return {PROP_NONE, GROUP_POOL};
 }
-static int is_f32_prop(int p)
-{
-    return (p >= N_F64 && p < N_F64 + N_F32) || (p >= B200SPH_VOL && p <= B200SPH_AP) || (p >= B200SPH_V00 && p <= B200SPH_AS22);
-}
-static double *f64_ptr(b200sph_ctx *ctx, int p)
-{
-    if (is_user_prop(p)) return ctx->user_f64[p - B200SPH_USER0];
-    return p < N_F64 ? ctx->f64[p] : (p < B200SPH_S00 ? ctx->f64x[p - B200SPH_UHAT] : ctx->f64s[p - B200SPH_S00]);
-}
-static float *f32_ptr(b200sph_ctx *ctx, int p)
-{
-    return p < N_F64 + N_F32 ? ctx->f32[p - N_F64] : (p < B200SPH_V00 ? ctx->f32x[p - B200SPH_VOL] : ctx->f32s[p - B200SPH_V00]);
-}
-static int u32_index(int p) { return (p >= B200SPH_GID && p <= B200SPH_PID) ? p - B200SPH_GID : -1; }
-// buffer k of the pool's main part (f64, f32, u32, f64x, f32x in that order) and its element size
-#define N_POOL (N_F64 + N_F32 + N_U32 + N_F64X + N_F32X)
-static void **pool_buf(b200sph_ctx *ctx, int k, size_t *esz)
-{
-    *esz = (k < N_F64 || (k >= N_F64 + N_F32 + N_U32 && k < N_POOL - N_F32X)) ? 8 : 4;
-    if (k < N_F64) return (void **)&ctx->f64[k];
-    if ((k -= N_F64) < N_F32) return (void **)&ctx->f32[k];
-    if ((k -= N_F32) < N_U32) return (void **)&ctx->u32[k];
-    if ((k -= N_U32) < N_F64X) return (void **)&ctx->f64x[k];
-    return (void **)&ctx->f32x[k - N_F64X];
-}
+static double *f64_ptr(const b200sph_ctx *ctx, int p) { return (double *)ctx->prop[p]; }
+static float *f32_ptr(const b200sph_ctx *ctx, int p) { return (float *)ctx->prop[p]; }
+static uint32_t *u32_ptr(const b200sph_ctx *ctx, int p) { return (uint32_t *)ctx->prop[p]; }
+static bool elastic_allocated(const b200sph_ctx *ctx) { return ctx->prop[B200SPH_S00] != nullptr; }
 
 // the neighbour lists can index n particles (26-bit sorted indices; beyond, and with
 // B200SPH_PAIR_KERNEL=warp, the list-free kernel runs)
@@ -723,11 +707,13 @@ static int pool_layout(b200sph_ctx *ctx, const int64_t *new_cap)
         total += (new_cap[a] + 31) / 32 * 32;
     }
     const int64_t alloc = std::max<int64_t>(total, 32);
-    // allocate new buffers and move array by array
-    for (int k = 0; k < N_POOL; k++) {
-        size_t esz;
-        void **slot = pool_buf(ctx, k, &esz);
-        void *old = *slot;
+    // allocate new buffers and move array by array: the pool's properties and those of the
+    // other groups that are allocated
+    for (int p = 0; p < N_PROP_SLOTS; p++) {
+        const PropKind pk = prop_kind(p);
+        if (pk.type == PROP_NONE || (pk.group != GROUP_POOL && !ctx->prop[p])) continue;
+        const size_t esz = pk.size();
+        void *old = ctx->prop[p];
         void *nw = nullptr;
         CU(cudaMalloc(&nw, esz * (size_t)alloc));
         CU(cudaMemsetAsync(nw, 0, esz * (size_t)alloc, ctx->stream));
@@ -742,42 +728,13 @@ static int pool_layout(b200sph_ctx *ctx, const int64_t *new_cap)
             CU(cudaStreamSynchronize(ctx->stream));
             CU(cudaFree(old));
         }
-        *slot = nw;
+        ctx->prop[p] = nw;
     }
-    if (ctx->solid_alloc) {   // the elastic-dynamics arrays move with the pool
-        for (int k = 0; k < 12 + 21; k++) {
-            const size_t esz = k < 12 ? 8 : 4;
-            void *old = k < 12 ? (void *)ctx->f64s[k] : (void *)ctx->f32s[k - 12];
-            void *nw = nullptr;
-            CU(cudaMalloc(&nw, esz * (size_t)alloc));
-            CU(cudaMemsetAsync(nw, 0, esz * (size_t)alloc, ctx->stream));
-            if (old) {
-                for (int a = 0; a < ctx->narr; a++)
-                    if (ctx->arr[a].n > 0 && ctx->arr[a].cap > 0)
-                        CU(cudaMemcpyAsync((char *)nw + esz * (size_t)new_off[a], (char *)old + esz * (size_t)ctx->arr[a].off,
-                                           esz * (size_t)ctx->arr[a].n, cudaMemcpyDeviceToDevice, ctx->stream));
-                CU(cudaStreamSynchronize(ctx->stream));
-                CU(cudaFree(old));
-            }
-            if (k < 12) ctx->f64s[k] = (double *)nw;
-            else ctx->f32s[k - 12] = (float *)nw;
-        }
+    if (elastic_allocated(ctx)) {
         for (float4 **r : {&ctx->T01, &ctx->T2R, &ctx->R2}) {
             if (*r) CU(cudaFree(*r));
             CU(cudaMalloc((void **)r, 16 * (size_t)alloc));
         }
-    }
-    for (int k = 0; k < B200SPH_MAX_USER; k++) {   // user properties move with the pool too
-        if (!ctx->user_f64[k]) continue;
-        double *old = ctx->user_f64[k], *nw = nullptr;
-        CU(cudaMalloc((void **)&nw, 8 * (size_t)alloc));
-        CU(cudaMemsetAsync(nw, 0, 8 * (size_t)alloc, ctx->stream));
-        for (int a = 0; a < ctx->narr; a++)
-            if (ctx->arr[a].n > 0 && ctx->arr[a].cap > 0)
-                CU(cudaMemcpyAsync(nw + new_off[a], old + ctx->arr[a].off, 8 * (size_t)ctx->arr[a].n, cudaMemcpyDeviceToDevice, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
-        CU(cudaFree(old));
-        ctx->user_f64[k] = nw;
     }
     if (ctx->ptype) CU(cudaFree(ctx->ptype));
     CU(cudaMalloc((void **)&ctx->ptype, (size_t)alloc));
@@ -960,8 +917,8 @@ template <class F> static int with_kernel_dim(b200sph_ctx *ctx, const char *who,
 // with the elastic-dynamics arrays allocated the deviatoric stress travels too: a ghost is a
 // source of group 2 (and, with SolidProgram.ghost_group1, a destination of group 1), and a
 // migrating particle takes s and its stage copy s0 along
-static inline int halo_nf(const b200sph_ctx *ctx) { return ctx->solid_alloc ? B200SPH_HALO_FIELDS_SOLID : B200SPH_HALO_FIELDS; }
-static inline int migrate_nf(const b200sph_ctx *ctx) { return ctx->solid_alloc ? B200SPH_MIGRATE_FIELDS_SOLID : B200SPH_MIGRATE_FIELDS; }
+static inline int halo_nf(const b200sph_ctx *ctx) { return elastic_allocated(ctx) ? B200SPH_HALO_FIELDS_SOLID : B200SPH_HALO_FIELDS; }
+static inline int migrate_nf(const b200sph_ctx *ctx) { return elastic_allocated(ctx) ? B200SPH_MIGRATE_FIELDS_SOLID : B200SPH_MIGRATE_FIELDS; }
 
 // the halo kernels are instantiated for either field count; `launch` gets it as
 // std::integral_constant<int, NF>
@@ -975,10 +932,10 @@ template <class F> static int with_halo_fields(const b200sph_ctx *ctx, F &&launc
 // kernel takes dt from the time-control block)
 template <class S> static void stage_args(b200sph_ctx *ctx, S &sa, int arr, int which, double dt, bool devdt)
 {
-    sa.x = ctx->f64[B200SPH_X]; sa.y = ctx->f64[B200SPH_Y]; sa.z = ctx->f64[B200SPH_Z];
-    sa.u = ctx->f64[B200SPH_U]; sa.v = ctx->f64[B200SPH_V]; sa.w = ctx->f64[B200SPH_W];
-    sa.x0 = ctx->f64[B200SPH_X0]; sa.y0 = ctx->f64[B200SPH_Y0]; sa.z0 = ctx->f64[B200SPH_Z0];
-    sa.u0 = ctx->f64[B200SPH_U0]; sa.v0 = ctx->f64[B200SPH_V0]; sa.w0 = ctx->f64[B200SPH_W0];
+    sa.x = f64_ptr(ctx, B200SPH_X); sa.y = f64_ptr(ctx, B200SPH_Y); sa.z = f64_ptr(ctx, B200SPH_Z);
+    sa.u = f64_ptr(ctx, B200SPH_U); sa.v = f64_ptr(ctx, B200SPH_V); sa.w = f64_ptr(ctx, B200SPH_W);
+    sa.x0 = f64_ptr(ctx, B200SPH_X0); sa.y0 = f64_ptr(ctx, B200SPH_Y0); sa.z0 = f64_ptr(ctx, B200SPH_Z0);
+    sa.u0 = f64_ptr(ctx, B200SPH_U0); sa.v0 = f64_ptr(ctx, B200SPH_V0); sa.w0 = f64_ptr(ctx, B200SPH_W0);
     sa.au = f32_ptr(ctx, B200SPH_AU); sa.av = f32_ptr(ctx, B200SPH_AV); sa.aw = f32_ptr(ctx, B200SPH_AW);
     sa.ax = f32_ptr(ctx, B200SPH_AX); sa.ay = f32_ptr(ctx, B200SPH_AY); sa.az = f32_ptr(ctx, B200SPH_AZ);
     sa.ptype = ctx->ptype;
@@ -994,7 +951,7 @@ template <class S> static void stage_args(b200sph_ctx *ctx, S &sa, int arr, int 
 // x0 .. rho0.  When the stage that follows will be the fused kernel, stage_impl only records it
 // (init_pending) and that kernel takes it as it goes (do_init): one sweep over the state less per
 // step.  Stage 1 of a context without ghosts does not even copy: the host exchanges the two sets
-// of buffers in ctx->f64 (init_by_rename), so that the state the initialize saw goes by
+// of buffers in ctx->prop (init_by_rename), so that the state the initialize saw goes by
 // x0 .. rho0 where it lies and the kernel writes the stepped state into the buffers that now go
 // by x .. rho (INIT_RENAMED); 56 B per particle less to write.  Otherwise the kernel copies
 // (INIT_COPY).  The one rule: whatever could observe the copy not being made yet -- reads x0 .. rho0,
@@ -1008,7 +965,7 @@ static int init_materialise(b200sph_ctx *ctx)
     ctx->init_pending = false;
     StageArgs sa;
     stage_args(ctx, sa, -1, 0, 0.0, false);
-    sa.rho = ctx->f64[B200SPH_RHO]; sa.rho0 = ctx->f64[B200SPH_RHO0]; sa.arho = f32_ptr(ctx, B200SPH_ARHO);
+    sa.rho = f64_ptr(ctx, B200SPH_RHO); sa.rho0 = f64_ptr(ctx, B200SPH_RHO0); sa.arho = f32_ptr(ctx, B200SPH_ARHO);
     if (ctx->pool_end > 0) {
         k_stage<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
         LAUNCH_CHECK();
@@ -1118,19 +1075,12 @@ int b200sph_destroy(b200sph_ctx *ctx)
     if (!ctx) return 0;
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    for (int k = 0; k < N_F64; k++) cudaFree(ctx->f64[k]);
-    for (int k = 0; k < N_F32; k++) cudaFree(ctx->f32[k]);
-    for (int k = 0; k < N_U32; k++) cudaFree(ctx->u32[k]);
-    for (int k = 0; k < N_F64X; k++) cudaFree(ctx->f64x[k]);
-    for (int k = 0; k < B200SPH_MAX_USER; k++) cudaFree(ctx->user_f64[k]);
+    for (void *b : ctx->prop) cudaFree(b);
     generic_unload_all(ctx);
-    for (int k = 0; k < N_F32X; k++) cudaFree(ctx->f32x[k]);
     cudaFree(ctx->Dv); cudaFree(ctx->PT); cudaFree(ctx->dfilter_F);
     for (auto &ps : ctx->probes) cudaFree(ps.xyz);
     cudaFree(ctx->interp_Q); cudaFree(ctx->interp_rho); cudaFree(ctx->interp_red); cudaFree(ctx->interp_out);
     for (auto &sg : ctx->mirror_segs) cudaFree(sg.idx);
-    for (int k = 0; k < 12; k++) cudaFree(ctx->f64s[k]);
-    for (int k = 0; k < 21; k++) cudaFree(ctx->f32s[k]);
     cudaFree(ctx->T01); cudaFree(ctx->T2R); cudaFree(ctx->R2);
     cudaFree(ctx->ptype);
     cudaFree(ctx->key_of); cudaFree(ctx->off_in); cudaFree(ctx->cell_cnt); cudaFree(ctx->cell_start);
@@ -1273,33 +1223,21 @@ static int ensure_stage(b200sph_ctx *ctx, int64_t count)
     return 0;
 }
 
-// user properties of the generic-equation fallback: allocated (zeroed) when first named
-static int ensure_user(b200sph_ctx *ctx, int prop)
+// a named elastic-dynamics or user property: allocated (zeroed) the first time anything names it,
+// the elastic-dynamics properties as one group with their stress records
+static int ensure_prop(b200sph_ctx *ctx, int prop)
 {
-    if (!is_user_prop(prop)) return 0;
-    double *&p = ctx->user_f64[prop - B200SPH_USER0];
-    if (p) return 0;
+    const PropGroup g = prop_kind(prop).group;
+    if (g == GROUP_POOL || ctx->prop[prop]) return 0;
     const size_t alloc = (size_t)std::max<int64_t>(ctx->pool_cap, 32);
-    CU(cudaMalloc((void **)&p, 8 * alloc));
-    CU(cudaMemsetAsync(p, 0, 8 * alloc, ctx->stream));
-    return 0;
-}
-
-// elastic-dynamics property arrays: allocated (zeroed) the first time anything names them
-static int ensure_solid(b200sph_ctx *ctx)
-{
-    if (ctx->solid_alloc) return 0;
-    const size_t alloc = (size_t)std::max<int64_t>(ctx->pool_cap, 32);
-    for (int k = 0; k < 12; k++) {
-        CU(cudaMalloc((void **)&ctx->f64s[k], 8 * alloc));
-        CU(cudaMemsetAsync(ctx->f64s[k], 0, 8 * alloc, ctx->stream));
+    for (int p = 0; p < N_PROP_SLOTS; p++) {
+        if (p != prop && (g == GROUP_USER || prop_kind(p).group != g)) continue;
+        const size_t esz = prop_kind(p).size();
+        CU(cudaMalloc(&ctx->prop[p], esz * alloc));
+        CU(cudaMemsetAsync(ctx->prop[p], 0, esz * alloc, ctx->stream));
     }
-    for (int k = 0; k < 21; k++) {
-        CU(cudaMalloc((void **)&ctx->f32s[k], 4 * alloc));
-        CU(cudaMemsetAsync(ctx->f32s[k], 0, 4 * alloc, ctx->stream));
-    }
-    for (float4 **r : {&ctx->T01, &ctx->T2R, &ctx->R2}) CU(cudaMalloc((void **)r, 16 * alloc));
-    ctx->solid_alloc = true;
+    if (g == GROUP_ELASTIC)
+        for (float4 **r : {&ctx->T01, &ctx->T2R, &ctx->R2}) CU(cudaMalloc((void **)r, 16 * alloc));
     return 0;
 }
 
@@ -1311,13 +1249,13 @@ int b200sph_push_f64(b200sph_ctx *ctx, int arr, int prop, const double *host, in
     if ((rc = check_range(ctx, arr, start, count))) return rc;
     // naming an elastic-dynamics property allocates that pool even for an empty array: every
     // rank of a slab decomposition must agree on the message layout (b200sph_halo_layout)
-    if (is_solid_prop(prop) && (rc = ensure_solid(ctx))) return rc;
-    if ((rc = ensure_user(ctx, prop))) return rc;
+    if ((rc = ensure_prop(ctx, prop))) return rc;
     if (count == 0) return 0;
     const int64_t o = ctx->arr[arr].off + start;
-    if (is_f64_prop(prop)) {
+    const PropType t = prop_kind(prop).type;
+    if (t == PROP_F64) {
         CU(cudaMemcpyAsync(f64_ptr(ctx, prop) + o, host, 8 * (size_t)count, cudaMemcpyHostToDevice, ctx->stream));
-    } else if (is_f32_prop(prop)) {
+    } else if (t == PROP_F32) {
         if ((rc = ensure_stage(ctx, count))) return rc;
         CU(cudaMemcpyAsync(ctx->stage_buf, host, 8 * (size_t)count, cudaMemcpyHostToDevice, ctx->stream));
         k_f64_to_f32<<<(unsigned)cdiv(count, 256), 256, 0, ctx->stream>>>(ctx->stage_buf, f32_ptr(ctx, prop) + o, count);
@@ -1347,11 +1285,11 @@ int b200sph_pull_f64(b200sph_ctx *ctx, int arr, int prop, double *host, int64_t 
     if ((rc = check_range(ctx, arr, start, count))) return rc;
     if (count == 0) return 0;
     const int64_t o = ctx->arr[arr].off + start;
-    if (is_solid_prop(prop) && (rc = ensure_solid(ctx))) return rc;
-    if ((rc = ensure_user(ctx, prop))) return rc;
-    if (is_f64_prop(prop)) {
+    if ((rc = ensure_prop(ctx, prop))) return rc;
+    const PropType t = prop_kind(prop).type;
+    if (t == PROP_F64) {
         CU(cudaMemcpyAsync(host, f64_ptr(ctx, prop) + o, 8 * (size_t)count, cudaMemcpyDeviceToHost, ctx->stream));
-    } else if (is_f32_prop(prop)) {
+    } else if (t == PROP_F32) {
         if ((rc = ensure_stage(ctx, count))) return rc;
         k_f32_to_f64<<<(unsigned)cdiv(count, 256), 256, 0, ctx->stream>>>(f32_ptr(ctx, prop) + o, ctx->stage_buf, count);
         LAUNCH_CHECK();
@@ -1369,10 +1307,9 @@ int b200sph_push_u32(b200sph_ctx *ctx, int arr, int prop, const uint32_t *host, 
     int rc = ensure_pool(ctx);
     if (rc) return rc;
     if ((rc = check_range(ctx, arr, start, count))) return rc;
-    const int k = u32_index(prop);
-    if (k < 0) return set_err(ctx, "push_u32: property id %d is not an integer property", prop);
+    if (prop_kind(prop).type != PROP_U32) return set_err(ctx, "push_u32: property id %d is not an integer property", prop);
     if (count == 0) return 0;
-    CU(cudaMemcpyAsync(ctx->u32[k] + ctx->arr[arr].off + start, host, 4 * (size_t)count, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(u32_ptr(ctx, prop) + ctx->arr[arr].off + start, host, 4 * (size_t)count, cudaMemcpyHostToDevice, ctx->stream));
     if (!ctx->async_copies) CU(cudaStreamSynchronize(ctx->stream));
     return 0;
 }
@@ -1384,10 +1321,9 @@ int b200sph_pull_u32(b200sph_ctx *ctx, int arr, int prop, uint32_t *host, int64_
     int rc = ensure_pool(ctx);
     if (rc) return rc;
     if ((rc = check_range(ctx, arr, start, count))) return rc;
-    const int k = u32_index(prop);
-    if (k < 0) return set_err(ctx, "pull_u32: property id %d is not an integer property", prop);
+    if (prop_kind(prop).type != PROP_U32) return set_err(ctx, "pull_u32: property id %d is not an integer property", prop);
     if (count == 0) return 0;
-    CU(cudaMemcpyAsync(host, ctx->u32[k] + ctx->arr[arr].off + start, 4 * (size_t)count, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(host, u32_ptr(ctx, prop) + ctx->arr[arr].off + start, 4 * (size_t)count, cudaMemcpyDeviceToHost, ctx->stream));
     if (!ctx->async_copies) CU(cudaStreamSynchronize(ctx->stream));
     return 0;
 }
@@ -1398,13 +1334,10 @@ int b200sph_device_ptr(b200sph_ctx *ctx, int arr, int prop, void **out)
     int rc = ensure_pool(ctx);
     if (rc) return rc;
     if (arr < 0 || arr >= ctx->narr) return set_err(ctx, "device_ptr: bad array %d", arr);
-    const int64_t o = ctx->arr[arr].off;
-    if (is_solid_prop(prop) && (rc = ensure_solid(ctx))) return rc;
-    if ((rc = ensure_user(ctx, prop))) return rc;
-    if (is_f64_prop(prop)) *out = f64_ptr(ctx, prop) + o;
-    else if (is_f32_prop(prop)) *out = f32_ptr(ctx, prop) + o;
-    else if (u32_index(prop) >= 0) *out = ctx->u32[u32_index(prop)] + o;
-    else return set_err(ctx, "device_ptr: bad property %d", prop);
+    if ((rc = ensure_prop(ctx, prop))) return rc;
+    const PropKind pk = prop_kind(prop);
+    if (pk.type == PROP_NONE) return set_err(ctx, "device_ptr: bad property %d", prop);
+    *out = (char *)ctx->prop[prop] + pk.size() * (size_t)ctx->arr[arr].off;
     return 0;
 }
 
@@ -1456,15 +1389,16 @@ int b200sph_snapshot_take(b200sph_ctx *ctx, int nseg, const int *arr, const int 
         }
         const int64_t o = ctx->arr[arr[i]].off;
         const int pr = prop[i];
-        if (is_solid_prop(pr) && (rc = ensure_solid(ctx))) return rc;
-        if (is_f64_prop(pr)) {
+        if ((rc = ensure_prop(ctx, pr))) return rc;
+        const PropType t = prop_kind(pr).type;
+        if (t == PROP_F64) {
             CU(cudaMemcpyAsync(dst, f64_ptr(ctx, pr) + o, 8 * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
-        } else if (is_f32_prop(pr)) {
+        } else if (t == PROP_F32) {
             k_f32_to_f64<<<(unsigned)cdiv(n, 256), 256, 0, ctx->stream>>>(f32_ptr(ctx, pr) + o, dst, n);
             LAUNCH_CHECK();
-        } else if (u32_index(pr) >= 0) {
+        } else if (t == PROP_U32) {
             ctx->snap_u32[i] = 1;
-            CU(cudaMemcpyAsync(dst, ctx->u32[u32_index(pr)] + o, 4 * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
+            CU(cudaMemcpyAsync(dst, u32_ptr(ctx, pr) + o, 4 * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
         } else {
             return set_err(ctx, "snapshot_take: bad property %d", pr);
         }
@@ -1519,8 +1453,8 @@ static int run_minmax(b200sph_ctx *ctx, int do_xyz, int do_h)
     ctx->dt_reduced = false;
     if (ctx->pool_end > 0) {
         const unsigned nb = (unsigned)std::min<int64_t>(cdiv(ctx->pool_end, 256), REDUCE_BLOCKS);
-        k_reduce_minmax<<<nb, 256, 0, ctx->stream>>>(ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z],
-                                                     ctx->f64[B200SPH_H], ctx->ptype, ctx->pool_end, do_xyz, do_h, ctx->red);
+        k_reduce_minmax<<<nb, 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_X), f64_ptr(ctx, B200SPH_Y), f64_ptr(ctx, B200SPH_Z),
+                                                     f64_ptr(ctx, B200SPH_H), ctx->ptype, ctx->pool_end, do_xyz, do_h, ctx->red);
         LAUNCH_CHECK();
     }
     CU(cudaMemcpyAsync(ctx->red_host, ctx->red, 16 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1537,7 +1471,7 @@ static int hm_uniformity(b200sph_ctx *ctx)
     CU(cudaMemcpyAsync(ctx->red, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
     if (ctx->pool_end > 0) {
         const unsigned nb = (unsigned)std::min<int64_t>(cdiv(ctx->pool_end, 256), REDUCE_BLOCKS);
-        k_reduce_minmax<<<nb, 256, 0, ctx->stream>>>(ctx->f64[B200SPH_H], ctx->f64[B200SPH_M], ctx->f64[B200SPH_M],
+        k_reduce_minmax<<<nb, 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_H), f64_ptr(ctx, B200SPH_M), f64_ptr(ctx, B200SPH_M),
                                                      nullptr, ctx->ptype, ctx->pool_end, 1, 0, ctx->red);
         LAUNCH_CHECK();
     }
@@ -1603,7 +1537,7 @@ int b200sph_update_domain(b200sph_ctx *ctx)
         }
         D.zorder = 0;
         if (ctx->pool_end > 0) {
-            k_box_wrap<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z],
+            k_box_wrap<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_X), f64_ptr(ctx, B200SPH_Y), f64_ptr(ctx, B200SPH_Z),
                                                                                    ctx->ptype, ctx->pool_end, D);
             LAUNCH_CHECK();
         }
@@ -1672,7 +1606,7 @@ static int pack_positions_light(b200sph_ctx *ctx, int clear)
 {
     if (clear) CU(cudaMemsetAsync(ctx->red_u32, 0, clear * sizeof(unsigned), ctx->stream));
     k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
-        ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H], ctx->perm, ctx->skey,
+        f64_ptr(ctx, B200SPH_X), f64_ptr(ctx, B200SPH_Y), f64_ptr(ctx, B200SPH_Z), f64_ptr(ctx, B200SPH_H), ctx->perm, ctx->skey,
         ctx->n_sorted, ctx->G, ctx->A0, ctx->A, ctx->AB, ctx->red_u32);
     ctx->ab_stale = false;   // (k_pack_pos_light writes the position half of AB)
     LAUNCH_CHECK();
@@ -1928,7 +1862,7 @@ int b200sph_nnps_update(b200sph_ctx *ctx)
     ctx->n_sorted = ntot;
     if (ctx->pool_end > 0) {
         const unsigned nb = (unsigned)cdiv(ctx->pool_end, 256);
-        k_cell_count<<<nb, 256, 0, ctx->stream>>>(ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z],
+        k_cell_count<<<nb, 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_X), f64_ptr(ctx, B200SPH_Y), f64_ptr(ctx, B200SPH_Z),
                                                   ctx->ptype, ctx->pool_end, G, ctx->key_of, ctx->off_in, ctx->cell_cnt);
         LAUNCH_CHECK();
     }
@@ -1940,7 +1874,7 @@ int b200sph_nnps_update(b200sph_ctx *ctx)
         const unsigned ns = (unsigned)cdiv(ntot, 256);
         k_canon<<<ns, 256, 0, ctx->stream>>>(ctx->perm_tmp, ctx->key_of, ctx->cell_start, ntot, ctx->perm, ctx->skey, ctx->rank);
         LAUNCH_CHECK();
-        k_pack_pos<<<ns, 256, 0, ctx->stream>>>(ctx->f64[B200SPH_X], ctx->f64[B200SPH_Y], ctx->f64[B200SPH_Z], ctx->f64[B200SPH_H],
+        k_pack_pos<<<ns, 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_X), f64_ptr(ctx, B200SPH_Y), f64_ptr(ctx, B200SPH_Z), f64_ptr(ctx, B200SPH_H),
                                                 ctx->perm, ctx->skey, ntot, G, ctx->A, ctx->AB, ctx->ptype, ctx->stype);
         LAUNCH_CHECK();
         if (use_lists)
@@ -2086,7 +2020,7 @@ static int eos_pool_flush(b200sph_ctx *ctx, cudaStream_t s)
 {
     if (!ctx->eos_pool_any) return 0;
     if (ctx->pool_end > 0) {
-        k_eos_tab<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, s>>>(ctx->f64[B200SPH_RHO], f32_ptr(ctx, B200SPH_P),
+        k_eos_tab<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, s>>>(f64_ptr(ctx, B200SPH_RHO), f32_ptr(ctx, B200SPH_P),
                                                                       f32_ptr(ctx, B200SPH_CS), ctx->ptype, ctx->pool_end, ctx->eos_pool);
         LAUNCH_CHECK();
     }
@@ -2110,7 +2044,7 @@ static int eos_flush(b200sph_ctx *ctx, cudaStream_t on_comm_stream)
     EosTab &E = ctx->eos_pending;
     if (ctx->pool_end > 0) {
         k_eos_tab<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, s>>>(
-            ctx->f64[B200SPH_RHO], f32_ptr(ctx, B200SPH_P), f32_ptr(ctx, B200SPH_CS), ctx->ptype, ctx->pool_end, E);
+            f64_ptr(ctx, B200SPH_RHO), f32_ptr(ctx, B200SPH_P), f32_ptr(ctx, B200SPH_CS), ctx->ptype, ctx->pool_end, E);
         LAUNCH_CHECK();
     }
     memset(E.on, 0, sizeof(E.on));
@@ -2124,7 +2058,7 @@ static int ab_positions(b200sph_ctx *ctx)
 {
     if (!ctx->ab_stale) return 0;
     if (ctx->n_sorted > 0) {
-        k_rec32_positions<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(ctx->R, ctx->f64[B200SPH_H], ctx->perm,
+        k_rec32_positions<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(ctx->R, f64_ptr(ctx, B200SPH_H), ctx->perm,
                                                                                        ctx->n_sorted, ctx->AB);
         LAUNCH_CHECK();
     }
@@ -2144,14 +2078,14 @@ static int pack_state(b200sph_ctx *ctx)
     if (ctx->rec32 && ctx->n_sorted > 0) {
         // (every particle is sorted: no ghosts, so the pool side of the EOS calls is complete)
         k_pack_rec32<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
-            ctx->f64[B200SPH_U], ctx->f64[B200SPH_V], ctx->f64[B200SPH_W], ctx->f64[B200SPH_RHO], f32_ptr(ctx, B200SPH_P),
+            f64_ptr(ctx, B200SPH_U), f64_ptr(ctx, B200SPH_V), f64_ptr(ctx, B200SPH_W), f64_ptr(ctx, B200SPH_RHO), f32_ptr(ctx, B200SPH_P),
             f32_ptr(ctx, B200SPH_CS), ctx->ptype, ctx->perm, ctx->n_sorted, ctx->AB, ctx->R, ctx->eos_pending, ctx->rec32_eos);
         LAUNCH_CHECK();
         memset(ctx->eos_pending.on, 0, sizeof(ctx->eos_pending.on));
         ctx->eos_any = false;
     } else if (ctx->n_sorted > 0) {
         k_pack_state<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
-            ctx->f64[B200SPH_U], ctx->f64[B200SPH_V], ctx->f64[B200SPH_W], ctx->f64[B200SPH_M], ctx->f64[B200SPH_RHO],
+            f64_ptr(ctx, B200SPH_U), f64_ptr(ctx, B200SPH_V), f64_ptr(ctx, B200SPH_W), f64_ptr(ctx, B200SPH_M), f64_ptr(ctx, B200SPH_RHO),
             f32_ptr(ctx, B200SPH_P), f32_ptr(ctx, B200SPH_CS), ctx->ptype, ctx->perm, ctx->n_sorted, ctx->B, ctx->C, ctx->AB,
             ctx->eos_pending, ctx->eos_any ? 1 : 0);
         LAUNCH_CHECK();
@@ -2244,7 +2178,7 @@ int b200sph_ferrari_h(b200sph_ctx *ctx, int arr, double hdx, int dim, int real_o
     if ((rc = arr_range(ctx, arr, real_only, &lo, &hi))) return rc;
     PhaseTimer pt(ctx, 2);
     if (hi > lo) {
-        k_ferrari<<<(unsigned)cdiv(hi - lo, 256), 256, 0, ctx->stream>>>(ctx->f64[B200SPH_H], ctx->f64[B200SPH_M], ctx->f64[B200SPH_RHO], lo, hi, hdx, 1.0 / dim);
+        k_ferrari<<<(unsigned)cdiv(hi - lo, 256), 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_H), f64_ptr(ctx, B200SPH_M), f64_ptr(ctx, B200SPH_RHO), lo, hi, hdx, 1.0 / dim);
         LAUNCH_CHECK();
     }
     h_changed(ctx);
@@ -2307,10 +2241,10 @@ static void generic_unload_all(b200sph_ctx *ctx)
 int b200sph_user_property(b200sph_ctx *ctx, int prop)
 {
     CU(cudaSetDevice(ctx->device));
-    if (!is_user_prop(prop)) return set_err(ctx, "user_property: ids %d..%d", B200SPH_USER0, B200SPH_USER0 + B200SPH_MAX_USER - 1);
+    if (prop_kind(prop).group != GROUP_USER) return set_err(ctx, "user_property: ids %d..%d", B200SPH_USER0, B200SPH_USER0 + B200SPH_MAX_USER - 1);
     int rc = ensure_pool(ctx);
     if (rc) return rc;
-    return ensure_user(ctx, prop);
+    return ensure_prop(ctx, prop);
 }
 
 int b200sph_generic_load(b200sph_ctx *ctx, const void *image, int64_t size)
@@ -2361,10 +2295,10 @@ int b200sph_generic_launch(b200sph_ctx *ctx, int module, const char *kernel, int
     }
     b200sph_generic_args ga;
     memset(&ga, 0, sizeof(ga));
-    for (int k = 0; k < N_F64; k++) ga.f64[k] = ctx->f64[k];
-    for (int k = 0; k < N_F32; k++) ga.f32[k] = ctx->f32[k];
-    for (int k = 0; k < N_U32; k++) ga.u32[k] = ctx->u32[k];
-    for (int k = 0; k < B200SPH_MAX_USER; k++) ga.user[k] = ctx->user_f64[k];
+    for (int k = 0; k < (int)std::size(ga.f64); k++) ga.f64[k] = f64_ptr(ctx, B200SPH_X + k);
+    for (int k = 0; k < (int)std::size(ga.f32); k++) ga.f32[k] = f32_ptr(ctx, B200SPH_P + k);
+    for (int k = 0; k < (int)std::size(ga.u32); k++) ga.u32[k] = u32_ptr(ctx, B200SPH_GID + k);
+    for (int k = 0; k < (int)std::size(ga.user); k++) ga.user[k] = f64_ptr(ctx, B200SPH_USER0 + k);
     ga.AB = ctx->AB; ga.stype = ctx->stype; ga.perm = ctx->perm;
     ga.cnt = ctx->cnt; ga.lst = ctx->lst; ga.capg = ctx->capg;
     ga.n = ctx->n_sorted;
@@ -2414,7 +2348,7 @@ int b200sph_density_filter(b200sph_ctx *ctx, uint32_t array_mask, int mode, int 
     if (mode == B200SPH_DFILTER_MLS2D && ctx->dim != 2) return set_err(ctx, "density_filter: MLSFirstOrder2D needs dim = 2 (dim is %d)", ctx->dim);
     if (mode == B200SPH_DFILTER_MLS3D && ctx->dim != 3) return set_err(ctx, "density_filter: MLSFirstOrder3D needs dim = 3 (dim is %d)", ctx->dim);
     if (array_mask == 0 || array_mask >= (1u << ctx->narr)) return set_err(ctx, "density_filter: bad array mask 0x%x", array_mask);
-    if (!is_user_prop(rhotmp_prop) || !ctx->user_f64[rhotmp_prop - B200SPH_USER0])
+    if (prop_kind(rhotmp_prop).group != GROUP_USER || !ctx->prop[rhotmp_prop])
         return set_err(ctx, "density_filter: rhotmp (property %d) is not a user property (b200sph_user_property)", rhotmp_prop);
     if (ctx->peer_box || ctx->comm_pending) return set_err(ctx, "density_filter runs on one GPU (no slab decomposition)");
     if (ctx->periodic[0] || ctx->periodic[1] || ctx->periodic[2] || mirror_any(ctx))
@@ -2441,7 +2375,7 @@ int b200sph_density_filter(b200sph_ctx *ctx, uint32_t array_mask, int mode, int 
         memset(&fa, 0, sizeof(fa));
         fa.AB = ctx->AB; fa.F = ctx->dfilter_F;
         fa.perm = ctx->perm; fa.cnt = ctx->cnt; fa.lst = ctx->lst; fa.stype = ctx->stype;
-        fa.m = ctx->f64[B200SPH_M]; fa.rho = ctx->f64[B200SPH_RHO]; fa.rhotmp = ctx->user_f64[rhotmp_prop - B200SPH_USER0];
+        fa.m = f64_ptr(ctx, B200SPH_M); fa.rho = f64_ptr(ctx, B200SPH_RHO); fa.rhotmp = f64_ptr(ctx, rhotmp_prop);
         fa.n = ctx->n_sorted; fa.capg = ctx->capg;
         fa.cellx = (float)ctx->G.cell[0]; fa.celly = (float)ctx->G.cell[1]; fa.cellz = (float)ctx->G.cell[2];
         const double kr = kernel_radius_scale(kernel);
@@ -2529,8 +2463,10 @@ int b200sph_interpolate(b200sph_ctx *ctx, int id, int method, int kernel, int di
     for (int a = 0; a < ctx->narr; a++) {
         const int p = props[a];
         if (p == -1 || !((array_mask >> a) & 1u)) continue;
-        if (is_f64_prop(p) && (!is_solid_prop(p) || ctx->solid_alloc) && f64_ptr(ctx, p)) ia.fd[a] = f64_ptr(ctx, p);
-        else if (is_f32_prop(p) && (p < B200SPH_V00 || ctx->solid_alloc) && f32_ptr(ctx, p)) ia.ff[a] = f32_ptr(ctx, p);
+        // a property without a buffer (nothing named it) is refused here, not allocated
+        const PropType t = prop_kind(p).type;
+        if (t == PROP_F64 && ctx->prop[p]) ia.fd[a] = f64_ptr(ctx, p);
+        else if (t == PROP_F32 && ctx->prop[p]) ia.ff[a] = f32_ptr(ctx, p);
         else return set_err(ctx, "interpolate: property id %d (array %d) is not a floating-point property of the pool", p, a);
     }
     int64_t ntot = 0;
@@ -2571,8 +2507,8 @@ int b200sph_interpolate(b200sph_ctx *ctx, int id, int method, int kernel, int di
     }
     {
         PhaseTimer pt(ctx, 2);
-        ia.x = ctx->f64[B200SPH_X]; ia.y = ctx->f64[B200SPH_Y]; ia.z = ctx->f64[B200SPH_Z];
-        ia.h = ctx->f64[B200SPH_H]; ia.m = ctx->f64[B200SPH_M]; ia.rho = ctx->f64[B200SPH_RHO];
+        ia.x = f64_ptr(ctx, B200SPH_X); ia.y = f64_ptr(ctx, B200SPH_Y); ia.z = f64_ptr(ctx, B200SPH_Z);
+        ia.h = f64_ptr(ctx, B200SPH_H); ia.m = f64_ptr(ctx, B200SPH_M); ia.rho = f64_ptr(ctx, B200SPH_RHO);
         ia.perm = ctx->perm; ia.skey = ctx->skey; ia.cell_start = ctx->cell_start; ia.stype = ctx->stype;
         ia.n = ctx->n_sorted;
         ia.G = ctx->G;
@@ -2752,7 +2688,7 @@ int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_
     pa.au = f32_ptr(ctx, B200SPH_AU); pa.av = f32_ptr(ctx, B200SPH_AV); pa.aw = f32_ptr(ctx, B200SPH_AW);
     pa.ax = f32_ptr(ctx, B200SPH_AX); pa.ay = f32_ptr(ctx, B200SPH_AY); pa.az = f32_ptr(ctx, B200SPH_AZ);
     pa.dt_cfl = f32_ptr(ctx, B200SPH_DT_CFL); pa.dt_force = f32_ptr(ctx, B200SPH_DT_FORCE);
-    pa.rho = ctx->f64[B200SPH_RHO];
+    pa.rho = f64_ptr(ctx, B200SPH_RHO);
     pa.n = ctx->n_sorted;
     pa.ncx = ctx->G.nc[0]; pa.ncy = ctx->G.nc[1]; pa.ncz = ctx->G.nc[2];
     pa.zorder = ctx->G.zorder;
@@ -2895,18 +2831,18 @@ int b200sph_tvf_pass(b200sph_ctx *ctx, const b200sph_tvf_program *prog, int64_t 
     // timing slots: pack + group 1 count as "other", group 2 (the dominant kernel) as "pair"
     std::unique_ptr<PhaseTimer> pt(new PhaseTimer(ctx, 2));
     const unsigned nbp = (unsigned)cdiv(ctx->n_sorted, 256);
-    k_pack_tvf<<<nbp, 256, 0, ctx->stream>>>(ctx->f64[B200SPH_U], ctx->f64[B200SPH_V], ctx->f64[B200SPH_W], ctx->f64[B200SPH_M],
+    k_pack_tvf<<<nbp, 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_U), f64_ptr(ctx, B200SPH_V), f64_ptr(ctx, B200SPH_W), f64_ptr(ctx, B200SPH_M),
                                              f64_ptr(ctx, B200SPH_UHAT), f64_ptr(ctx, B200SPH_VHAT),
                                              f64_ptr(ctx, B200SPH_WHAT), f64_ptr(ctx, B200SPH_PF),
                                              f32_ptr(ctx, B200SPH_PAVG), ctx->ptype, ctx->perm, ctx->n_sorted,
-                                             ctx->B, ctx->AB, ctx->C, ctx->Dv, ctx->PT, ctx->f64[B200SPH_RHO], solid_mask);
+                                             ctx->B, ctx->AB, ctx->C, ctx->Dv, ctx->PT, f64_ptr(ctx, B200SPH_RHO), solid_mask);
     LAUNCH_CHECK();
     state_changed(ctx);   // B / C no longer hold the WCSPH records
 
     TvfArgs ta;
     memset(&ta, 0, sizeof(ta));
     ta.AB = ctx->AB; ta.C2 = ctx->C; ta.Dv = ctx->Dv; ta.PT = ctx->PT; ta.perm = ctx->perm;
-    ta.rho = ctx->f64[B200SPH_RHO];
+    ta.rho = f64_ptr(ctx, B200SPH_RHO);
     ta.V = f32_ptr(ctx, B200SPH_VOL); ta.pavg = f32_ptr(ctx, B200SPH_PAVG);
     ta.au = f32_ptr(ctx, B200SPH_AU); ta.av = f32_ptr(ctx, B200SPH_AV); ta.aw = f32_ptr(ctx, B200SPH_AW);
     ta.auhat = f32_ptr(ctx, B200SPH_AUHAT); ta.avhat = f32_ptr(ctx, B200SPH_AVHAT);
@@ -2971,7 +2907,7 @@ int b200sph_solid_pass(b200sph_ctx *ctx, const b200sph_solid_program *prog, int6
     int rc = ensure_pool(ctx);
     if (rc) return rc;
     if ((rc = eos_flush(ctx))) return rc;
-    if ((rc = ensure_solid(ctx))) return rc;
+    if ((rc = ensure_prop(ctx, B200SPH_S00))) return rc;
     if (!ctx->grid_valid) return set_err(ctx, "solid_pass: the NNPS is stale (particles were pushed/resized); call nnps_update first");
     if (!(prog->passes & 3)) return set_err(ctx, "solid_pass: passes must select group 1 and/or group 2");
     if (prog->elastic_mask == 0 || prog->elastic_mask >= (1u << ctx->narr)) return set_err(ctx, "solid_pass: bad elastic mask 0x%x", prog->elastic_mask);
@@ -2982,13 +2918,13 @@ int b200sph_solid_pass(b200sph_ctx *ctx, const b200sph_solid_program *prog, int6
     SolidArgs sa;
     memset(&sa, 0, sizeof(sa));
     sa.AB = ctx->AB; sa.C3 = ctx->C; sa.T01 = ctx->T01; sa.T2R = ctx->T2R; sa.R2 = ctx->R2; sa.perm = ctx->perm;
-    sa.rho = ctx->f64[B200SPH_RHO];
+    sa.rho = f64_ptr(ctx, B200SPH_RHO);
     for (int k = 0; k < 6; k++) {
-        sa.s[k] = ctx->f64s[k];
-        sa.r[k] = ctx->f32s[9 + k];
-        sa.as[k] = ctx->f32s[15 + k];
+        sa.s[k] = f64_ptr(ctx, B200SPH_S00 + k);
+        sa.r[k] = f32_ptr(ctx, B200SPH_R00 + k);
+        sa.as[k] = f32_ptr(ctx, B200SPH_AS00 + k);
     }
-    for (int k = 0; k < 9; k++) sa.vg[k] = ctx->f32s[k];
+    for (int k = 0; k < 9; k++) sa.vg[k] = f32_ptr(ctx, B200SPH_V00 + k);
     sa.p = f32_ptr(ctx, B200SPH_P);
     sa.arho = f32_ptr(ctx, B200SPH_ARHO);
     sa.au = f32_ptr(ctx, B200SPH_AU); sa.av = f32_ptr(ctx, B200SPH_AV); sa.aw = f32_ptr(ctx, B200SPH_AW);
@@ -3012,7 +2948,7 @@ int b200sph_solid_pass(b200sph_ctx *ctx, const b200sph_solid_program *prog, int6
     if (prog->passes & 1) {
         // group 2 alone reuses the records the last group 1 left behind
         k_pack_solid<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
-            ctx->f64[B200SPH_U], ctx->f64[B200SPH_V], ctx->f64[B200SPH_W], ctx->f64[B200SPH_M], ctx->f64[B200SPH_RHO],
+            f64_ptr(ctx, B200SPH_U), f64_ptr(ctx, B200SPH_V), f64_ptr(ctx, B200SPH_W), f64_ptr(ctx, B200SPH_M), f64_ptr(ctx, B200SPH_RHO),
             f32_ptr(ctx, B200SPH_P), f32_ptr(ctx, B200SPH_CS), ctx->ptype, ctx->perm, ctx->n_sorted, ctx->B, ctx->AB, ctx->C);
         LAUNCH_CHECK();
         state_changed(ctx);   // B / C no longer hold the WCSPH records
@@ -3058,15 +2994,15 @@ static int stage_begin(b200sph_ctx *ctx, const char *who, int arr, int which, bo
 static int stage_solid_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devdt)
 {
     int rc = stage_begin(ctx, "stage_solid", arr, which, devdt);
-    if (rc || (rc = ensure_solid(ctx))) return rc;
+    if (rc || (rc = ensure_prop(ctx, B200SPH_S00))) return rc;
     PhaseTimer pt(ctx, 2);
     StageSolidArgs sa;
     stage_args(ctx, sa, arr, which, dt, devdt);
-    sa.rho = ctx->f64[B200SPH_RHO]; sa.rho0 = ctx->f64[B200SPH_RHO0]; sa.arho = f32_ptr(ctx, B200SPH_ARHO);
+    sa.rho = f64_ptr(ctx, B200SPH_RHO); sa.rho0 = f64_ptr(ctx, B200SPH_RHO0); sa.arho = f32_ptr(ctx, B200SPH_ARHO);
     for (int k = 0; k < 6; k++) {
-        sa.s[k] = ctx->f64s[k];
-        sa.s0[k] = ctx->f64s[6 + k];
-        sa.as[k] = ctx->f32s[15 + k];
+        sa.s[k] = f64_ptr(ctx, B200SPH_S00 + k);
+        sa.s0[k] = f64_ptr(ctx, B200SPH_S000 + k);
+        sa.as[k] = f32_ptr(ctx, B200SPH_AS00 + k);
     }
     if (ctx->pool_end > 0) {
         k_stage_solid<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
@@ -3142,18 +3078,18 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
     PhaseTimer pt(ctx, 2);
     int do_init = ctx->init_pending ? INIT_COPY : INIT_NONE;
     if (which != 0 && fused && ctx->init_pending && init_by_rename(ctx, which)) {
-        for (int k = 0; k <= B200SPH_RHO - B200SPH_X; k++) std::swap(ctx->f64[B200SPH_X + k], ctx->f64[B200SPH_X0 + k]);
+        for (int k = 0; k <= B200SPH_RHO - B200SPH_X; k++) std::swap(ctx->prop[B200SPH_X + k], ctx->prop[B200SPH_X0 + k]);
         do_init = INIT_RENAMED;
     }
     StageArgs sa;
     stage_args(ctx, sa, arr, which, dt, devdt);
     if (rk3) sa.f = dt;   // every TVD-RK3 stage takes the whole dt
-    sa.rho = ctx->f64[B200SPH_RHO]; sa.rho0 = ctx->f64[B200SPH_RHO0]; sa.arho = f32_ptr(ctx, B200SPH_ARHO);
+    sa.rho = f64_ptr(ctx, B200SPH_RHO); sa.rho0 = f64_ptr(ctx, B200SPH_RHO0); sa.arho = f32_ptr(ctx, B200SPH_ARHO);
     if (which != 0 && fused) {
         // stage + records of the next evaluation (+ the dt factors after the last stage) in one pass
         FusePackArgs q;
         memset(&q, 0, sizeof(q));
-        q.h = ctx->f64[B200SPH_H]; q.m = ctx->f64[B200SPH_M];
+        q.h = f64_ptr(ctx, B200SPH_H); q.m = f64_ptr(ctx, B200SPH_M);
         q.p = f32_ptr(ctx, B200SPH_P); q.cs = f32_ptr(ctx, B200SPH_CS);
         q.rank = ctx->rank; q.key_of = ctx->key_of;
         q.A0 = ctx->A0; q.AB = ctx->AB; q.C = ctx->C;
@@ -3252,7 +3188,7 @@ static int reduce_dt_factors(b200sph_ctx *ctx)
     LAUNCH_CHECK();
     if (ctx->pool_end > 0) {
         const unsigned nb = (unsigned)std::min<int64_t>(cdiv(ctx->pool_end, 256), REDUCE_BLOCKS);
-        k_reduce_dt<<<nb, 256, 0, ctx->stream>>>(f32_ptr(ctx, B200SPH_DT_CFL), f32_ptr(ctx, B200SPH_DT_FORCE), ctx->f64[B200SPH_H],
+        k_reduce_dt<<<nb, 256, 0, ctx->stream>>>(f32_ptr(ctx, B200SPH_DT_CFL), f32_ptr(ctx, B200SPH_DT_FORCE), f64_ptr(ctx, B200SPH_H),
                                                  ctx->ptype, ctx->pool_end, ctx->red);
         LAUNCH_CHECK();
     }
@@ -3367,15 +3303,57 @@ int b200sph_dt_factors(b200sph_ctx *ctx, double out[3])
 }
 
 // ---- halo helpers ------------------------------------------------------------
-static const int halo_fields[9] = {B200SPH_X, B200SPH_Y, B200SPH_Z, B200SPH_U, B200SPH_V, B200SPH_W, B200SPH_RHO, B200SPH_H, B200SPH_M};
+// The ghost and the migration message by property id, field by field: the first halo_nf /
+// migrate_nf of these (the elastic-dynamics fields travel only when that group is allocated).
+// An fp32 or integer property travels as a double.
+static const int halo_msg[B200SPH_HALO_FIELDS_SOLID] = {
+    B200SPH_X, B200SPH_Y, B200SPH_Z, B200SPH_U, B200SPH_V, B200SPH_W, B200SPH_RHO, B200SPH_H, B200SPH_M,
+    B200SPH_S00, B200SPH_S01, B200SPH_S02, B200SPH_S11, B200SPH_S12, B200SPH_S22, B200SPH_CS};
+static const int migrate_msg[B200SPH_MIGRATE_FIELDS_SOLID] = {
+    B200SPH_X, B200SPH_Y, B200SPH_Z, B200SPH_U, B200SPH_V, B200SPH_W, B200SPH_RHO, B200SPH_H, B200SPH_M,
+    B200SPH_X0, B200SPH_Y0, B200SPH_Z0, B200SPH_U0, B200SPH_V0, B200SPH_W0, B200SPH_RHO0, B200SPH_GID,
+    B200SPH_S00, B200SPH_S01, B200SPH_S02, B200SPH_S11, B200SPH_S12, B200SPH_S22,
+    B200SPH_S000, B200SPH_S010, B200SPH_S020, B200SPH_S110, B200SPH_S120, B200SPH_S220, B200SPH_CS};
 
+// the halo kernels' view of the ghost message: its fp64 fields, then cs
 static HaloPtrs halo_ptrs(b200sph_ctx *ctx)
 {
     HaloPtrs P;
-    for (int f = 0; f < B200SPH_HALO_FIELDS; f++) P.p[f] = ctx->f64[halo_fields[f]];
-    for (int f = B200SPH_HALO_FIELDS; f < B200SPH_HALO_FIELDS_SOLID - 1; f++) P.p[f] = ctx->f64s[f - B200SPH_HALO_FIELDS];
-    P.cs = f32_ptr(ctx, B200SPH_CS);
+    for (int f = 0; f < B200SPH_HALO_FIELDS_SOLID - 1; f++) P.p[f] = f64_ptr(ctx, halo_msg[f]);
+    P.cs = f32_ptr(ctx, halo_msg[B200SPH_HALO_FIELDS_SOLID - 1]);
     return P;
+}
+
+// zero particles [o, o + n) of the allocated properties among ids first .. last
+static int zero_props(b200sph_ctx *ctx, int first, int last, int64_t o, int64_t n)
+{
+    for (int p = first; p <= last; p++) {
+        const size_t esz = prop_kind(p).size();
+        if (ctx->prop[p]) CU(cudaMemsetAsync((char *)ctx->prop[p] + esz * (size_t)o, 0, esz * (size_t)n, ctx->stream));
+    }
+    return 0;
+}
+
+// What the particles [o, o + n) that arrive by a message get for the properties it does not carry:
+// the derived fp32 fields (of the elastic-dynamics group too, when it is allocated) zero; with the
+// ghost message (no stage copies, no gid) the stage copies zero and gid 0xFFFFFFFF; tag `tag`; pid 0.
+// Called before the message is written: an elastic array's cs comes with it.
+static int arrival_init(b200sph_ctx *ctx, int64_t o, int64_t n, bool ghost_msg, uint32_t tag)
+{
+    const unsigned nb = (unsigned)cdiv(n, 256);
+    int rc;
+    if ((rc = zero_props(ctx, B200SPH_P, B200SPH_DT_FORCE, o, n)) || (rc = zero_props(ctx, B200SPH_V00, B200SPH_AS22, o, n)))
+        return rc;
+    if (ghost_msg) {
+        if ((rc = zero_props(ctx, B200SPH_X0, B200SPH_RHO0, o, n)) || (rc = zero_props(ctx, B200SPH_S000, B200SPH_S220, o, n)))
+            return rc;
+        k_fill_u32<<<nb, 256, 0, ctx->stream>>>(u32_ptr(ctx, B200SPH_GID) + o, n, 0xFFFFFFFFu);
+        LAUNCH_CHECK();
+    }
+    k_fill_u32<<<nb, 256, 0, ctx->stream>>>(u32_ptr(ctx, B200SPH_TAG) + o, n, tag);
+    LAUNCH_CHECK();
+    CU(cudaMemsetAsync(u32_ptr(ctx, B200SPH_PID) + o, 0, 4 * (size_t)n, ctx->stream));
+    return 0;
 }
 
 // ---- mirror boundaries ----------------------------------------------------------------
@@ -3403,7 +3381,7 @@ static int mirror_refresh(b200sph_ctx *ctx)
 static int mirror_create(b200sph_ctx *ctx)
 {
     int rc;
-    if (ctx->solid_alloc) return set_err(ctx, "mirror boundaries: images carry the WCSPH fields only (x y z u v w rho h m), not the elastic-dynamics state");
+    if (elastic_allocated(ctx)) return set_err(ctx, "mirror boundaries: images carry the WCSPH fields only (x y z u v w rho h m), not the elastic-dynamics state");
     if ((rc = eos_flush(ctx))) return rc;
     // the cell size of the REAL particles decides the width (images have their sources' h)
     for (int a = 0; a < ctx->narr; a++) ctx->arr[a].n = ctx->arr[a].n_real;
@@ -3425,7 +3403,7 @@ static int mirror_create(b200sph_ctx *ctx)
                 sg.ghost_first = ai.n - ai.n_real;
                 if (n_sel == 0) continue;
                 const unsigned nb = (unsigned)cdiv(n_sel + 1, 256);
-                k_flag_mirror<<<nb, 256, 0, ctx->stream>>>(ctx->f64[B200SPH_X + axis], ai.off, n_sel, side == 0 ? ctx->dom_lo[axis] : ctx->dom_hi[axis], width, side, ctx->flag_a);
+                k_flag_mirror<<<nb, 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_X + axis), ai.off, n_sel, side == 0 ? ctx->dom_lo[axis] : ctx->dom_hi[axis], width, side, ctx->flag_a);
                 LAUNCH_CHECK();
                 if ((rc = device_scan(ctx, ctx->flag_a, ctx->flag_b, n_sel + 1))) return rc;
                 uint32_t tot = 0;
@@ -3441,17 +3419,10 @@ static int mirror_create(b200sph_ctx *ctx)
                 LAUNCH_CHECK();
                 if ((rc = ensure_capacity(ctx, a, ai.n + tot))) return rc;   // may move the pool
                 const int64_t o = ai.off + ai.n;
-                const unsigned nbt = (unsigned)cdiv((int64_t)tot, 256);
-                k_mirror_copy<<<nbt, 256, 0, ctx->stream>>>(halo_ptrs(ctx), ai.off, sg.idx, (long long)tot, o, axis, 2.0 * (side == 0 ? ctx->dom_lo[axis] : ctx->dom_hi[axis]));
+                // images arrive like ghosts, with tag = Ghost (2)
+                if ((rc = arrival_init(ctx, o, tot, true, 2u))) return rc;
+                k_mirror_copy<<<(unsigned)cdiv((int64_t)tot, 256), 256, 0, ctx->stream>>>(halo_ptrs(ctx), ai.off, sg.idx, (long long)tot, o, axis, 2.0 * (side == 0 ? ctx->dom_lo[axis] : ctx->dom_hi[axis]));
                 LAUNCH_CHECK();
-                // like halo_append for ghosts: stage copies and derived fields zero, no gid, tag = Ghost (2)
-                for (int k = B200SPH_X0; k < N_F64; k++) CU(cudaMemsetAsync(ctx->f64[k] + o, 0, 8 * (size_t)tot, ctx->stream));
-                for (int k = 0; k < N_F32; k++) CU(cudaMemsetAsync(ctx->f32[k] + o, 0, 4 * (size_t)tot, ctx->stream));
-                k_fill_u32<<<nbt, 256, 0, ctx->stream>>>(ctx->u32[0] + o, tot, 0xFFFFFFFFu);
-                LAUNCH_CHECK();
-                k_fill_u32<<<nbt, 256, 0, ctx->stream>>>(ctx->u32[1] + o, tot, 2u);
-                LAUNCH_CHECK();
-                CU(cudaMemsetAsync(ctx->u32[2] + o, 0, 4 * (size_t)tot, ctx->stream));
                 sg.count = tot;
                 ai.n += tot;
             }
@@ -3483,7 +3454,7 @@ int b200sph_halo_pack(b200sph_ctx *ctx, int arr, int slot, double lo, double hi,
     if (slot == 0 || slot == 1) ctx->halo_cnt[arr][slot] = 0;
     if (n == 0) return 0;
     const unsigned nb = (unsigned)cdiv(n + 1, 256);
-    k_flag_range<<<nb, 256, 0, ctx->stream>>>(ctx->f64[B200SPH_X], off, n, lo, hi, 0, ctx->flag_a);
+    k_flag_range<<<nb, 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_X), off, n, lo, hi, 0, ctx->flag_a);
     LAUNCH_CHECK();
     if ((rc = device_scan(ctx, ctx->flag_a, ctx->flag_b, n + 1))) return rc;
     uint32_t tot = 0;
@@ -3528,11 +3499,8 @@ int b200sph_halo_append(b200sph_ctx *ctx, int arr, const double *dev_buf, int64_
     if ((rc = ensure_capacity(ctx, arr, ai.n + n))) return rc;
     const int64_t o = ai.off + ai.n;
     const unsigned nb = (unsigned)cdiv(n, 256);
-    // derived fields of the appended particles start at zero (cs of an elastic array is then
-    // filled from the message)
-    for (int k = 0; k < N_F32; k++) CU(cudaMemsetAsync(ctx->f32[k] + o, 0, 4 * (size_t)n, ctx->stream));
-    if (ctx->solid_alloc)
-        for (int k = 0; k < 21; k++) CU(cudaMemsetAsync(ctx->f32s[k] + o, 0, 4 * (size_t)n, ctx->stream));
+    // tag = Remote (1) for ghosts
+    if ((rc = arrival_init(ctx, o, n, nfields == hnf, as_real ? 0u : 1u))) return rc;
     if (nfields == hnf) {
         rc = with_halo_fields(ctx, [&](auto nf) {
             k_halo_scatter<decltype(nf)::value><<<nb, 256, 0, ctx->stream>>>(halo_ptrs(ctx), o, dev_buf, stride, n);
@@ -3540,27 +3508,20 @@ int b200sph_halo_append(b200sph_ctx *ctx, int arr, const double *dev_buf, int64_
             return 0;
         });
         if (rc) return rc;
-        for (int k = B200SPH_X0; k < N_F64; k++) CU(cudaMemsetAsync(ctx->f64[k] + o, 0, 8 * (size_t)n, ctx->stream));
-        if (ctx->solid_alloc)
-            for (int k = 6; k < 12; k++) CU(cudaMemsetAsync(ctx->f64s[k] + o, 0, 8 * (size_t)n, ctx->stream));
-        k_fill_u32<<<nb, 256, 0, ctx->stream>>>(ctx->u32[0] + o, n, 0xFFFFFFFFu);
-        LAUNCH_CHECK();
     } else {
-        for (int k = 0; k < N_F64; k++)
-            CU(cudaMemcpyAsync(ctx->f64[k] + o, dev_buf + (size_t)k * stride, 8 * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
-        k_f64_to_u32<<<nb, 256, 0, ctx->stream>>>(dev_buf + (size_t)N_F64 * stride, ctx->u32[0] + o, n);
-        LAUNCH_CHECK();
-        if (ctx->solid_alloc) {  // fields 17..28: s00..s22, s000..s220; field 29: cs
-            for (int k = 0; k < 12; k++)
-                CU(cudaMemcpyAsync(ctx->f64s[k] + o, dev_buf + (size_t)(B200SPH_MIGRATE_FIELDS + k) * stride, 8 * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
-            k_f64_to_f32<<<nb, 256, 0, ctx->stream>>>(dev_buf + (size_t)(B200SPH_MIGRATE_FIELDS + 12) * stride, f32_ptr(ctx, B200SPH_CS) + o, n);
+        for (int f = 0; f < mnf; f++) {
+            const int p = migrate_msg[f];
+            const double *src = dev_buf + (size_t)f * stride;
+            const PropType t = prop_kind(p).type;
+            if (t == PROP_F64) {
+                CU(cudaMemcpyAsync(f64_ptr(ctx, p) + o, src, 8 * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
+                continue;
+            }
+            if (t == PROP_F32) k_f64_to_f32<<<nb, 256, 0, ctx->stream>>>(src, f32_ptr(ctx, p) + o, n);
+            else k_f64_to_u32<<<nb, 256, 0, ctx->stream>>>(src, u32_ptr(ctx, p) + o, n);
             LAUNCH_CHECK();
         }
     }
-    // tag = Remote (1) for ghosts
-    k_fill_u32<<<nb, 256, 0, ctx->stream>>>(ctx->u32[1] + o, n, as_real ? 0u : 1u);
-    LAUNCH_CHECK();
-    CU(cudaMemsetAsync(ctx->u32[2] + o, 0, 4 * (size_t)n, ctx->stream));
     ai.n += n;
     if (as_real) ai.n_real += n;
     set_changed_with_h(ctx);
@@ -3921,7 +3882,7 @@ int b200sph_peer_recv(b200sph_ctx *ctx, int side, const int64_t *ghost_first, co
     const bool repack = ctx->packed_valid && reusable_build(ctx) && ctx->n_sorted > 0;
     // the ghosts' state records too when the real particles' are in place (fused stage kernel;
     // WCSPH records: not with the elastic-dynamics arrays)
-    const bool records = repack && ctx->state_packed && !ctx->solid_alloc;
+    const bool records = repack && ctx->state_packed && !elastic_allocated(ctx);
     GhostPackArgs R;
     memset(&R, 0, sizeof(R));
     R.rank = repack ? ctx->rank : nullptr;
@@ -4056,7 +4017,7 @@ int b200sph_column_counts(b200sph_ctx *ctx, int arr, double x0, double inv_width
     const ArrayInfo &ai = ctx->arr[arr];
     if (ai.n_real == 0) return 0;
     const unsigned nb = (unsigned)cdiv(cdiv(ai.n_real, COLUMN_RUN), 256);
-    k_column_counts<<<nb, 256, 0, ctx->stream>>>(ctx->f64[B200SPH_X], ai.off, ai.n_real, x0, inv_width, nbins, dev_counts);
+    k_column_counts<<<nb, 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_X), ai.off, ai.n_real, x0, inv_width, nbins, dev_counts);
     LAUNCH_CHECK();
     return 0;
 }
@@ -4078,7 +4039,7 @@ int b200sph_migrate_out(b200sph_ctx *ctx, int arr, double lo, double hi, double 
     const int mnf = migrate_nf(ctx);
     int64_t base = 0;  // doubles written so far
     for (int side = 0; side < 2; side++) {
-        k_flag_range<<<nb, 256, 0, ctx->stream>>>(ctx->f64[B200SPH_X], off, n, lo, hi, side == 0 ? 1 : 2, ctx->flag_a);
+        k_flag_range<<<nb, 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_X), off, n, lo, hi, side == 0 ? 1 : 2, ctx->flag_a);
         LAUNCH_CHECK();
         if ((rc = device_scan(ctx, ctx->flag_a, ctx->flag_b, n + 1))) return rc;
         uint32_t tot = 0;
@@ -4086,51 +4047,33 @@ int b200sph_migrate_out(b200sph_ctx *ctx, int arr, double lo, double hi, double 
         CU(cudaStreamSynchronize(ctx->stream));
         count[side] = tot;
         if (base + (int64_t)tot * mnf > cap * mnf) return set_err(ctx, "migrate_out: buffer too small");
-        if (tot) {
-            for (int k = 0; k < N_F64; k++) {
-                k_gather_f64<<<nb, 256, 0, ctx->stream>>>(ctx->f64[k], off, n, ctx->flag_a, ctx->flag_b, dev_buf, base + (long long)k * tot);
-                LAUNCH_CHECK();
-            }
-            k_gather_u32_as_f64<<<nb, 256, 0, ctx->stream>>>(ctx->u32[0], off, n, ctx->flag_a, ctx->flag_b, dev_buf, base + (long long)N_F64 * tot);
+        for (int f = 0; tot && f < mnf; f++) {
+            const int p = migrate_msg[f];
+            const long long at = base + (long long)f * tot;
+            const PropType t = prop_kind(p).type;
+            if (t == PROP_F64) k_gather_f64<<<nb, 256, 0, ctx->stream>>>(f64_ptr(ctx, p), off, n, ctx->flag_a, ctx->flag_b, dev_buf, at);
+            else if (t == PROP_F32) k_gather_f32_as_f64<<<nb, 256, 0, ctx->stream>>>(f32_ptr(ctx, p), off, n, ctx->flag_a, ctx->flag_b, dev_buf, at);
+            else k_gather_u32_as_f64<<<nb, 256, 0, ctx->stream>>>(u32_ptr(ctx, p), off, n, ctx->flag_a, ctx->flag_b, dev_buf, at);
             LAUNCH_CHECK();
-            if (ctx->solid_alloc) {
-                for (int k = 0; k < 12; k++) {
-                    k_gather_f64<<<nb, 256, 0, ctx->stream>>>(ctx->f64s[k], off, n, ctx->flag_a, ctx->flag_b, dev_buf, base + (long long)(B200SPH_MIGRATE_FIELDS + k) * tot);
-                    LAUNCH_CHECK();
-                }
-                k_gather_f32_as_f64<<<nb, 256, 0, ctx->stream>>>(f32_ptr(ctx, B200SPH_CS), off, n, ctx->flag_a, ctx->flag_b, dev_buf, base + (long long)(B200SPH_MIGRATE_FIELDS + 12) * tot);
-                LAUNCH_CHECK();
-            }
         }
         base += (int64_t)tot * mnf;
     }
     if (count[0] + count[1] == 0) return 0;
     // stable compaction of the keepers, property by property, through the staging buffer
-    k_flag_range<<<nb, 256, 0, ctx->stream>>>(ctx->f64[B200SPH_X], off, n, lo, hi, 3, ctx->flag_a);
+    k_flag_range<<<nb, 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_X), off, n, lo, hi, 3, ctx->flag_a);
     LAUNCH_CHECK();
     if ((rc = device_scan(ctx, ctx->flag_a, ctx->flag_b, n + 1))) return rc;
     const int64_t keep = n - count[0] - count[1];
     if ((rc = ensure_stage(ctx, n))) return rc;
-    // x is the selection key: compact it last
-    for (int k = N_F64 - 1; k >= 0; k--) {
-        k_gather_f64<<<nb, 256, 0, ctx->stream>>>(ctx->f64[k], off, n, ctx->flag_a, ctx->flag_b, ctx->stage_buf, 0);
+    // the keepers keep what the migration message carries, and tag and pid (the other fp32
+    // fields are recomputed); 4-byte properties move as bits
+    for (int f = 0; f < mnf + 2; f++) {
+        const int p = f < mnf ? migrate_msg[f] : (f == mnf ? B200SPH_TAG : B200SPH_PID);
+        const size_t esz = prop_kind(p).size();
+        if (esz == 8) k_gather_f64<<<nb, 256, 0, ctx->stream>>>(f64_ptr(ctx, p), off, n, ctx->flag_a, ctx->flag_b, ctx->stage_buf, 0);
+        else k_gather_u32<<<nb, 256, 0, ctx->stream>>>(u32_ptr(ctx, p), off, n, ctx->flag_a, ctx->flag_b, (uint32_t *)ctx->stage_buf);
         LAUNCH_CHECK();
-        if (keep) CU(cudaMemcpyAsync(ctx->f64[k] + off, ctx->stage_buf, 8 * (size_t)keep, cudaMemcpyDeviceToDevice, ctx->stream));
-    }
-    for (int k = 0; k < N_U32; k++) {
-        k_gather_u32<<<nb, 256, 0, ctx->stream>>>(ctx->u32[k], off, n, ctx->flag_a, ctx->flag_b, (uint32_t *)ctx->stage_buf);
-        LAUNCH_CHECK();
-        if (keep) CU(cudaMemcpyAsync(ctx->u32[k] + off, ctx->stage_buf, 4 * (size_t)keep, cudaMemcpyDeviceToDevice, ctx->stream));
-    }
-    if (ctx->solid_alloc) {  // the keepers' stress state and cs move with them (the other fp32 fields are recomputed)
-        for (int k = 0; k < 12; k++) {
-            k_gather_f64<<<nb, 256, 0, ctx->stream>>>(ctx->f64s[k], off, n, ctx->flag_a, ctx->flag_b, ctx->stage_buf, 0);
-            LAUNCH_CHECK();
-            if (keep) CU(cudaMemcpyAsync(ctx->f64s[k] + off, ctx->stage_buf, 8 * (size_t)keep, cudaMemcpyDeviceToDevice, ctx->stream));
-        }
-        k_gather_u32<<<nb, 256, 0, ctx->stream>>>((const uint32_t *)f32_ptr(ctx, B200SPH_CS), off, n, ctx->flag_a, ctx->flag_b, (uint32_t *)ctx->stage_buf);
-        LAUNCH_CHECK();
-        if (keep) CU(cudaMemcpyAsync(f32_ptr(ctx, B200SPH_CS) + off, ctx->stage_buf, 4 * (size_t)keep, cudaMemcpyDeviceToDevice, ctx->stream));
+        if (keep) CU(cudaMemcpyAsync((char *)ctx->prop[p] + esz * (size_t)off, ctx->stage_buf, esz * (size_t)keep, cudaMemcpyDeviceToDevice, ctx->stream));
     }
     ai.n = ai.n_real = keep;
     set_changed_with_h(ctx);

@@ -330,6 +330,95 @@ def test_push_pull_roundtrip_and_errors(gpu_device):
             pass
         pb.B200AccelerationEval([pa], [Foo(dest='f', sources=['f'])],
                                 pb.CubicSpline(dim=2), backend=be)
+    # every property id through every entry point that names one
+    f64 = set(range(0, 16)) | set(range(27, 32)) | set(range(70, 82)) | set(range(110, 126))
+    f32 = set(range(16, 27)) | set(range(32, 38)) | set(range(82, 103))
+    u32 = {64, 65, 66}
+    accepts = dict(push_f64=f64 | f32, pull_f64=f64 | f32, push_u32=u32, pull_u32=u32,
+                   device_ptr=f64 | f32 | u32, snapshot=f64 | f32 | u32)
+    for entry, ids in accepts.items():
+        rows, init = property_id_sweep(entry)
+        assert [p for p, ok, _, _, _ in rows if ok] == sorted(ids), entry
+        for p, ok, before, after, out in rows:
+            # naming an elastic-dynamics property (70 .. 102) allocates the group: the ghost and
+            # migration messages grow from 9 / 17 to 16 / 30 fields
+            grows = entry not in ('push_u32', 'pull_u32')
+            assert before == ((16, 30) if grows and p > 70 else (9, 17)), (entry, p)
+            assert after == ((16, 30) if grows and p >= 70 else (9, 17)), (entry, p)
+            if not ok:
+                continue
+            if entry == 'device_ptr':
+                assert out, p
+                continue
+            if entry == 'push_f64':
+                want = p + np.arange(5) / 3.0
+            elif entry == 'push_u32':
+                want = 1000 * p + np.arange(5)
+            else:   # what the context was created with; zeros for what it was not given
+                want = init.get(p, np.zeros(5))
+            if p in f32:
+                want = np.asarray(want, dtype=np.float32)
+            assert np.array_equal(out, want), (entry, p, out, want)
+
+
+SWEEP_IDS = list(range(-1, 127)) + [130, 255, 1 << 20]
+
+
+def property_id_sweep(entry, skip=()):
+    """What one entry point does with every property id in SWEEP_IDS (ascending), on a fresh
+    context over one 5-particle array: rows (id, accepted, b200sph_halo_layout before and after,
+    the values a push_f64 / pull_f64 or push_u32 / pull_u32 round trip, a pull or a one-segment
+    snapshot returns, or whether device_ptr gave a pointer), and the values the context was
+    created with, by id."""
+    import ctypes as C
+    import pysph_b200 as pb
+    from pysph_b200._lib import B200Error, INT_PROP_IDS
+    n = 5
+    rs = np.random.RandomState(11)
+    pa = pb.get_particle_array_wcsph(name='f', x=np.zeros(n))
+    for k, a in pa.properties.items():
+        a[:] = np.arange(n) + 7 if a.dtype.kind in 'iu' else rs.uniform(-2, 2, n)
+    be = pb.B200Backend([pa])
+    ids = dict(be.prop_ids[0], **INT_PROP_IDS)
+    init = dict((ids[k], a.copy()) for k, a in pa.properties.items() if k in ids)
+    call = be.ctx.call
+
+    def layout():
+        h, m = C.c_int(), C.c_int()
+        call('b200sph_halo_layout', C.byref(h), C.byref(m))
+        return h.value, m.value
+    rows = []
+    for p in SWEEP_IDS:
+        if p in skip:
+            continue
+        before = layout()
+        out = np.zeros(n, dtype=np.uint32 if entry.endswith('u32') else np.float64)
+        try:
+            if entry == 'push_f64':
+                v = p + np.arange(n) / 3.0
+                call('b200sph_push_f64', 0, p, v.ctypes.data, 0, n)
+            elif entry == 'push_u32':
+                v = (1000 * p + np.arange(n)).astype(np.uint32)
+                call('b200sph_push_u32', 0, p, v.ctypes.data, 0, n)
+            if entry == 'device_ptr':
+                ptr = C.c_void_p()
+                call('b200sph_device_ptr', 0, p, C.byref(ptr))
+                out = ptr.value is not None
+            elif entry == 'snapshot':
+                call('b200sph_snapshot_take', 1, (C.c_int * 1)(0), (C.c_int * 1)(p),
+                     (C.c_int64 * 1)(n))
+                if p in INT_PROP_IDS.values():
+                    out = out.astype(np.uint32)
+                call('b200sph_snapshot_fetch', 0, out.ctypes.data, n)
+                call('b200sph_snapshot_release')
+            else:
+                call('b200sph_pull_' + entry[-3:], 0, p, out.ctypes.data, 0, n)
+            ok = True
+        except B200Error:
+            ok, out = False, None
+        rows.append((p, ok, before, layout(), out))
+    be.ctx.close()
+    return rows, init
 
 
 def test_determinism(gpu_device):
