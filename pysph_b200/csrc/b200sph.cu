@@ -38,7 +38,6 @@
 #include <cstring>
 #include <iterator>
 #include <string>
-#include <memory>
 #include <mutex>
 #include <type_traits>
 #include <vector>
@@ -870,13 +869,17 @@ struct PhaseTimer {
     b200sph_ctx *ctx;
     int slot;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
-    PhaseTimer(b200sph_ctx *c, int s);
-    ~PhaseTimer();
+    PhaseTimer(b200sph_ctx *c, int s) : ctx(c) { start(s); }
+    ~PhaseTimer() { stop(); }
+    void to(int s) { stop(); start(s); }   // ends this phase; what follows is timed into slot s
+    void start(int s);
+    void stop();
 };
 
 
-PhaseTimer::PhaseTimer(b200sph_ctx *c, int s) : ctx(c), slot(s)
+void PhaseTimer::start(int s)
 {
+    slot = s;
     if (!ctx->profiling || (ctx->profiling == 2 && slot != 1)) return;
     for (cudaEvent_t *e : {&e0, &e1}) {
         if (!ctx->ev_pool.empty()) {
@@ -888,11 +891,12 @@ PhaseTimer::PhaseTimer(b200sph_ctx *c, int s) : ctx(c), slot(s)
     }
     cudaEventRecord(e0, ctx->stream);
 }
-PhaseTimer::~PhaseTimer()
+void PhaseTimer::stop()
 {
     if (!e0) return;
     cudaEventRecord(e1, ctx->stream);
     ctx->pending.push_back({e0, e1, slot});
+    e0 = e1 = nullptr;
 }
 
 // The (kernel, dim) pairs the templated pair-walking kernels are instantiated for: every kernel
@@ -2829,7 +2833,7 @@ int b200sph_tvf_pass(b200sph_ctx *ctx, const b200sph_tvf_program *prog, int64_t 
     if ((rc = prepare_lists(ctx, nullptr, "tvf_pass: the EDAC kernels need the neighbour-list path (B200SPH_PAIR_KERNEL=list, < 2^26 particles)")))
         return rc;
     // timing slots: pack + group 1 count as "other", group 2 (the dominant kernel) as "pair"
-    std::unique_ptr<PhaseTimer> pt(new PhaseTimer(ctx, 2));
+    PhaseTimer pt(ctx, 2);
     const unsigned nbp = (unsigned)cdiv(ctx->n_sorted, 256);
     k_pack_tvf<<<nbp, 256, 0, ctx->stream>>>(f64_ptr(ctx, B200SPH_U), f64_ptr(ctx, B200SPH_V), f64_ptr(ctx, B200SPH_W), f64_ptr(ctx, B200SPH_M),
                                              f64_ptr(ctx, B200SPH_UHAT), f64_ptr(ctx, B200SPH_VHAT),
@@ -2873,10 +2877,7 @@ int b200sph_tvf_pass(b200sph_ctx *ctx, const b200sph_tvf_program *prog, int64_t 
     // stages: 1 group 1 (fluids), 2 group 1 (wall arrays), 3 the average-pressure group, 4 group 2
     for (int stage = 1; stage <= 4; stage++) {
         const int pass = stage == 4 ? 2 : 1;
-        if (stage == 4) {
-            pt.reset();
-            pt.reset(new PhaseTimer(ctx, 1));
-        }
+        if (stage == 4) pt.to(1);
         if (stage == 1 && !(prog->passes & 1)) continue;
         if (stage == 2 && !((prog->passes & 1) && solid_mask)) continue;
         if (stage == 3 && !(prog->passes & 4)) continue;
@@ -2897,7 +2898,7 @@ int b200sph_tvf_pass(b200sph_ctx *ctx, const b200sph_tvf_program *prog, int64_t 
         if (stage == 3) ta.bql = prog->bql;
         if (pass == 2) ctx->stats.pair_launches++;
     }
-    pt.reset();
+    pt.stop();
     return pairs_read(ctx, pairs_out);
 }
 
@@ -2944,7 +2945,7 @@ int b200sph_solid_pass(b200sph_ctx *ctx, const b200sph_solid_program *prog, int6
         sa.wdeltap[a] = (float)prog->wdeltap[a]; sa.nexp[a] = (float)prog->n[a];
     }
     if ((rc = pairs_arm(ctx, pairs_out, &sa.pair_counter))) return rc;
-    std::unique_ptr<PhaseTimer> pt(new PhaseTimer(ctx, 2));
+    PhaseTimer pt(ctx, 2);
     if (prog->passes & 1) {
         // group 2 alone reuses the records the last group 1 left behind
         k_pack_solid<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
@@ -2955,10 +2956,7 @@ int b200sph_solid_pass(b200sph_ctx *ctx, const b200sph_solid_program *prog, int6
     }
     const unsigned nb = (unsigned)cdiv(ctx->n_sorted, LIST_NT);
     for (int pass = 1; pass <= 2; pass++) {
-        if (pass == 2) {
-            pt.reset();
-            pt.reset(new PhaseTimer(ctx, 1));
-        }
+        if (pass == 2) pt.to(1);
         if (!(prog->passes & pass)) continue;
         rc = with_kernel_dim(ctx, "solid_pass", [&](auto kc, auto dc) {
             constexpr int K = decltype(kc)::value, D = decltype(dc)::value;
@@ -2970,7 +2968,7 @@ int b200sph_solid_pass(b200sph_ctx *ctx, const b200sph_solid_program *prog, int6
         if (rc) return rc;
         if (pass == 2) ctx->stats.pair_launches++;
     }
-    pt.reset();
+    pt.stop();
     return pairs_read(ctx, pairs_out);
 }
 

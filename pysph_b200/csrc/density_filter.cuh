@@ -109,18 +109,15 @@ __global__ void __launch_bounds__(DFILTER_NT) k_density_filter(const DensityFilt
     int cmax = count;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) cmax = max(cmax, __shfl_xor_sync(FULL, cmax, o));
-    const uint32_t *nxt = a.lst + ((size_t)(s >> 5) * (size_t)a.capg) * 32u + (uint32_t)(s & 31);
+    const uint32_t *nxt = list_slot(a.lst, a.capg, s);
     const float hi2 = a.k2 * Ai.w * Ai.w;
     struct Rec { float4 A, B; };
     const auto load = [&](const uint32_t e, Rec &r) { ld_256(a.F + 2u * LIST_J(e), r.A, r.B); };
     // W_ij of a list entry, 0 unless the pair passes the exact accept test and the source is of
     // the destination's array (the lists may hold other arrays' entries for other passes)
     const auto weight = [&](const bool live, const uint32_t e, const Rec &r, float &xij, float &yij, float &zij) {
-        const float4 T = list_cell_offset(e, a.cellx, a.celly, a.cellz);
-        xij = Ai.x - r.A.x + T.x, yij = Ai.y - r.A.y + T.y, zij = Ai.z - r.A.z + T.z;
-        const float r2 = xij * xij + yij * yij + zij * zij;
-        const bool take = live && ((r2 < hi2) || (r2 < a.k2 * r.A.w * r.A.w)) &&
-                          ((__float_as_int(r.B.z) & 7) == (ti & 7));
+        const float r2 = list_dist(e, a.cellx, a.celly, a.cellz, Ai, r.A, xij, yij, zij);
+        const bool take = live && NNPS_ACCEPT(r2, hi2, a.k2, r.A.w) && ((__float_as_int(r.B.z) & 7) == (ti & 7));
         const float rinv = r2 > 1e-24f ? frsqrt(r2) : 0.0f;      // RIJ > 1e-12 guard, kernels.py:128-132
         const float h1 = frcp(0.5f * (Ai.w + r.A.w));
         float w, dw;

@@ -451,7 +451,7 @@ __global__ void __launch_bounds__(LIST_NT) k_chunk_classify(const uint32_t *__re
     if (s < n) {
         hit = sflag[s];
         const int count = (int)cnt[s];
-        const uint32_t *my = lst + ((size_t)(s >> 5) * (size_t)capg) * 32u + (uint32_t)(s & 31);
+        const uint32_t *my = list_slot(lst, capg, s);
         for (int k = 0; k < count && !hit; k++) hit = sflag[LIST_J(my[(size_t)k * 32u])];
     }
     __shared__ int s_hit;

@@ -55,6 +55,21 @@ struct Acc {
     float arho, au, av, aw, ax, ay, az, cfl, rsum;
 };
 
+// The neighbour search's exact accept test, linked_list_nnps.pyx:188: (xij2 < hi2) or (xij2 < hj2),
+// hi2 = (k h_i)^2 formed once per destination.  A macro, not a function: inlined from a function,
+// the || is flattened into a predicated OR, and the kernels that test it get other code.
+#define NNPS_ACCEPT(r2, hi2, k2, hj) ((r2) < (hi2) || (r2) < (k2) * (hj) * (hj))
+
+// adds the pairs the lanes of a warp took to the evaluation's pair counter a.pair_counter (null:
+// not counted)
+template <class Args> __device__ __forceinline__ void pairs_flush(const Args &a, unsigned npairs)
+{
+    if (!a.pair_counter) return;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) npairs += __shfl_xor_sync(0xffffffffu, npairs, o);
+    if ((threadIdx.x & 31) == 0 && npairs) atomicAdd(a.pair_counter, (unsigned long long)npairs);
+}
+
 // EQS: what the Group can contain, known when the kernel is chosen -- the low 8 bits are the
 // equation bits that may occur, PAIR_EQS_TENSILE that the tensile correction may be on.
 // The default admits everything; a narrower set lets the compiler drop the other
@@ -214,8 +229,7 @@ __global__ void __launch_bounds__(PAIR_WARPS * 32) k_pair(const PairArgs a)
                     zij = zoff - Aj.z;
                     hj = Aj.w;
                     const float r2 = xij * xij + yij * yij + zij * zij;
-                    // linked_list_nnps.pyx:188: (xij2 < hi2) or (xij2 < hj2)
-                    ok = (r2 < hi2) || (r2 < a.k2 * hj * hj);
+                    ok = NNPS_ACCEPT(r2, hi2, a.k2, hj);
                 }
                 const unsigned m = __ballot_sync(FULL, ok);
                 if (m) {
@@ -280,9 +294,5 @@ __global__ void __launch_bounds__(PAIR_WARPS * 32) k_pair(const PairArgs a)
             }
         }
     }
-    if (a.pair_counter) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) npairs += __shfl_xor_sync(FULL, npairs, o);
-        if (lane == 0 && npairs) atomicAdd(a.pair_counter, (unsigned long long)npairs);
-    }
+    pairs_flush(a, npairs);
 }

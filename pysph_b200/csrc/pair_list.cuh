@@ -25,6 +25,14 @@
 #define LIST_J(e) ((uint32_t)(e) >> LIST_CBITS)
 #define LIST_CODE(e) ((uint32_t)(e) & 63u)
 #define LIST_NT 128
+
+// entry 0 of destination s in the transposed lists (capg entries reserved per destination); its
+// entry k is 32 k further on
+template <class T> __device__ __forceinline__ T *list_slot(T *lst, const int capg, const long long s)
+{
+    return lst + ((size_t)(s >> 5) * (size_t)capg) * 32u + (uint32_t)(s & 31);
+}
+
 // Skin controller.  Per evaluation a build costs c0 (1+s)^3 (list entries) + R / L(s)
 // (rebuild cost R over a lifetime L that grows linearly with the skin s); the minimum is
 // where L s = R / (3 c0 (1+s)^2) ~ 2 for the measured R / c0 ~ 5.5, i.e. the target
@@ -93,7 +101,7 @@ __global__ void __launch_bounds__(LB_WARPS * 32) k_list_build(const ListBuildArg
     }
     const float hi = a.kr * Ai.w + a.S;
     const float hi2 = hi * hi;
-    uint32_t *out = (a.lst && valid) ? a.lst + ((size_t)(s >> 5) * (size_t)a.capg) * 32u + (uint32_t)(s & 31) : nullptr;
+    uint32_t *out = (a.lst && valid) ? list_slot(a.lst, a.capg, s) : nullptr;
     unsigned count = 0;
     // the lanes of a warp usually share one cell row; at a row end they are served row by row
     unsigned todo = __ballot_sync(FULL, valid);
@@ -236,38 +244,26 @@ __device__ __forceinline__ void list_walk(const uint32_t *nxt, const int count, 
     }
 }
 
-// the cell offset a list entry carries, as the vector to ADD to (x_i - x_j) of cell-relative
-// coordinates: -(d - 1) * cell per axis, d the 2-bit code field.  (code field | 0x4B000000) as a
-// float is 2^23 + field exactly, so the decode is one LOP3 + one FADD per axis; a shared-memory
-// table of the 64 vectors cost 16 % of the LSU data-pipe wavefronts in k_pair_list.
-__device__ __forceinline__ float4 list_cell_offset(const uint32_t e, const float cellx, const float celly, const float cellz)
+// x_ij of list entry e, from cell-relative positions Ai (destination) and Aj (source) and the
+// offset of the source's cell the entry carries, and its square r^2.  Every list consumer uses
+// this one expression, so all of them take the same accept decisions on the same positions.
+// The offset is -(d - 1) * cell per axis, d the 2-bit code field, decoded arithmetically:
+// (code field | 0x4B000000) as a float is 2^23 + field, exactly, so d - 1 costs one LOP3 and
+// one FADD per axis; a shared-memory table of the 64 offset vectors cost 16 % of the LSU
+// data-pipe wavefronts in k_pair_list.
+__device__ __forceinline__ float list_dist(const uint32_t e, const float cellx, const float celly, const float cellz,
+                                           const float4 Ai, const float4 Aj, float &xij, float &yij, float &zij)
 {
     const float dxc = __uint_as_float((e & 3u) | 0x4B000000u) - 8388609.0f;
     const float dyc = __uint_as_float(((e >> 2) & 3u) | 0x4B000000u) - 8388609.0f;
     const float dzc = __uint_as_float(((e >> 4) & 3u) | 0x4B000000u) - 8388609.0f;
-    return make_float4(-dxc * cellx, -dyc * celly, -dzc * cellz, 0.f);
-}
-
-// one list entry: cell-offset lookup, distance, the exact accept test, the equations.  `live`
-// is false for the lanes whose list is shorter than the warp's longest (their entry reads
-// as 0 and their record as record 0, so everything up to the test is harmless to execute).
-// x_ij of a list entry and its square; both list consumers of the WCSPH Group use this one
-// expression, so that they take the same accept decisions on the same positions
-__device__ __forceinline__ float entry_dist(const PairArgs &a, const uint32_t e, const float4 Ai, const float4 Aj,
-                                            float &xij, float &yij, float &zij)
-{
-    // cell offset of the neighbour's cell relative to the destination's, decoded arithmetically:
-    // (code field | 0x4B000000) as a float is 2^23 + field, exactly, so field - 1 costs one
-    // LOP3 and one FADD per axis, where a shared-memory table of the 64 offset vectors would
-    // add divergent 128-bit reads to the load pipe the gathers already use.
-    const float dxc = __uint_as_float((e & 3u) | 0x4B000000u) - 8388609.0f;
-    const float dyc = __uint_as_float(((e >> 2) & 3u) | 0x4B000000u) - 8388609.0f;
-    const float dzc = __uint_as_float(((e >> 4) & 3u) | 0x4B000000u) - 8388609.0f;
-    xij = fmaf(-dxc, a.cellx, Ai.x - Aj.x), yij = fmaf(-dyc, a.celly, Ai.y - Aj.y),
-    zij = fmaf(-dzc, a.cellz, Ai.z - Aj.z);
+    xij = fmaf(-dxc, cellx, Ai.x - Aj.x), yij = fmaf(-dyc, celly, Ai.y - Aj.y), zij = fmaf(-dzc, cellz, Ai.z - Aj.z);
     return xij * xij + yij * yij + zij * zij;
 }
 
+// one list entry: distance, the exact accept test, the equations.  `live` is false for the
+// lanes whose list is shorter than the warp's longest (their entry reads as 0 and their record
+// as record 0, so everything up to the test is harmless to execute).
 template <int K, int DIM, int EQS>
 __device__ __forceinline__ void pair_entry(const PairArgs &a, const bool live, const uint32_t e,
                                            const float4 Aj, const float4 Bj, const float4 Cj, const float4 Ai,
@@ -275,9 +271,8 @@ __device__ __forceinline__ void pair_entry(const PairArgs &a, const bool live, c
                                            const unsigned long long mask_i, Acc &acc, unsigned &npairs)
 {
     float xij, yij, zij;
-    const float r2 = entry_dist(a, e, Ai, Aj, xij, yij, zij);
-    // the exact accept test, linked_list_nnps.pyx:188
-    if (live && ((r2 < hi2) || (r2 < a.k2 * Aj.w * Aj.w)))
+    const float r2 = list_dist(e, a.cellx, a.celly, a.cellz, Ai, Aj, xij, yij, zij);
+    if (live && NNPS_ACCEPT(r2, hi2, a.k2, Aj.w))
         pair_body<K, DIM, EQS>(a, make_float4(xij, yij, zij, Aj.w), Bj, Cj, Ai, Bi, Ci, mask_i, Ci.y, acc, npairs);
 }
 
@@ -312,7 +307,7 @@ __global__ void __launch_bounds__(LIST_NT, MINB) k_pair_list(const PairArgs a, c
     int cmax = count;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) cmax = max(cmax, __shfl_xor_sync(FULL, cmax, o));
-    const uint32_t *nxt = lst + ((size_t)(s >> 5) * (size_t)capg) * 32u + (uint32_t)(s & 31);
+    const uint32_t *nxt = list_slot(lst, capg, s);
     const float hi2 = a.k2 * Ai.w * Ai.w;
     Acc acc = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     unsigned npairs = 0;
@@ -343,11 +338,7 @@ __global__ void __launch_bounds__(LIST_NT, MINB) k_pair_list(const PairArgs a, c
             a.ax[g] = acc.ax + Bi.x; a.ay[g] = acc.ay + Bi.y; a.az[g] = acc.az + Bi.z;
         }
     }
-    if (a.pair_counter) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) npairs += __shfl_xor_sync(FULL, npairs, o);
-        if ((tid & 31) == 0 && npairs) atomicAdd(a.pair_counter, (unsigned long long)npairs);
-    }
+    pairs_flush(a, npairs);
 }
 
 // The list consumer of the 32-byte records (records32 in b200sph.cu: the WCSPH scheme's Group
@@ -382,8 +373,10 @@ __global__ void __launch_bounds__(LIST_NT, 8) k_pair_list_r32(const PairArgs a, 
     int cmax = count;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) cmax = max(cmax, __shfl_xor_sync(FULL, cmax, o));
-    const uint32_t *nxt = lst + ((size_t)(s >> 5) * (size_t)capg) * 32u + (uint32_t)(s & 31);
-    const float h2k = a.k2 * a.h * a.h;          // k_pair_list's hi2 (and hj2) on the same floats
+    const uint32_t *nxt = list_slot(lst, capg, s);
+    // k_pair_list's hi2 (and hj2) on the same floats: h is uniform, so the accept test is one
+    // compare, r2 < h2k, where NNPS_ACCEPT would make two on equal bounds
+    const float h2k = a.k2 * a.h * a.h;
     const float xi = 1.0f + Vi.w;
     const float tmpi = Pi.w;                                             // p_i / rho_i^2
     const float aci = a.ac0 * (xi * xi * xi);                            // -alpha cs_i / 2
@@ -397,9 +390,9 @@ __global__ void __launch_bounds__(LIST_NT, 8) k_pair_list_r32(const PairArgs a, 
         [&](const uint32_t e, Rec &r) { ld_256(a.R + 2u * LIST_J(e), r.P, r.V); },
         [&](const bool live, const uint32_t e, const Rec &r) {
             float xij, yij, zij;
-            const float r2 = entry_dist(a, e, Pi, r.P, xij, yij, zij);
-            // the exact accept test, linked_list_nnps.pyx:188, then the Group's equations for the
-            // source's type (none: the pair is not counted); without ghosts the type is the array
+            const float r2 = list_dist(e, a.cellx, a.celly, a.cellz, Pi, r.P, xij, yij, zij);
+            // the exact accept test, then the Group's equations for the source's type (none: the
+            // pair is not counted); without ghosts the type is the array
             const unsigned eq = (live && r2 < h2k) ? sel >> (__float_as_int(r.V.w) & 7) : 0u;
             const bool c_on = eq & (1u << ESEL_CONTINUITY), m_on = eq & (1u << ESEL_MOMENTUM), x_on = eq & (1u << ESEL_XSPH);
             npairs += (eq >> ESEL_ANY) & 1u;
@@ -449,9 +442,5 @@ __global__ void __launch_bounds__(LIST_NT, 8) k_pair_list_r32(const PairArgs a, 
             a.ax[g] = fmaf(me, acc.ax, Vi.x); a.ay[g] = fmaf(me, acc.ay, Vi.y); a.az[g] = fmaf(me, acc.az, Vi.z);
         }
     }
-    if (a.pair_counter) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) npairs += __shfl_xor_sync(FULL, npairs, o);
-        if ((tid & 31) == 0 && npairs) atomicAdd(a.pair_counter, (unsigned long long)npairs);
-    }
+    pairs_flush(a, npairs);
 }

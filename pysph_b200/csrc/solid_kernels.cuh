@@ -122,7 +122,7 @@ __global__ void __launch_bounds__(LIST_NT, 4) k_solid_pass1(const SolidArgs a, c
     int cmax = count;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) cmax = max(cmax, __shfl_xor_sync(FULL, cmax, o));
-    const uint32_t *my = lst + ((size_t)(s >> 5) * (size_t)capg) * 32u + (uint32_t)(s & 31);
+    const uint32_t *my = list_slot(lst, capg, s);
     const float hi2 = a.k2 * Ai.w * Ai.w;
     float g00 = 0.f, g01 = 0.f, g02 = 0.f, g10 = 0.f, g11 = 0.f, g12 = 0.f, g20 = 0.f, g21 = 0.f, g22 = 0.f;
     unsigned npairs = 0;
@@ -135,10 +135,9 @@ __global__ void __launch_bounds__(LIST_NT, 4) k_solid_pass1(const SolidArgs a, c
         },
         [&](const bool live, const uint32_t e, const Rec &r) {
             const float4 Aj = r.A, Bj = r.B, Cj = r.C;
-            const float4 T = list_cell_offset(e, a.cellx, a.celly, a.cellz);
-            const float xij = Ai.x - Aj.x + T.x, yij = Ai.y - Aj.y + T.y, zij = Ai.z - Aj.z + T.z;
-            const float r2 = xij * xij + yij * yij + zij * zij;
-            if (live && ((r2 < hi2) || (r2 < a.k2 * Aj.w * Aj.w)) && ((a.source_mask >> (__float_as_int(Cj.w) & 7)) & 1u)) {
+            float xij, yij, zij;
+            const float r2 = list_dist(e, a.cellx, a.celly, a.cellz, Ai, Aj, xij, yij, zij);
+            if (live && NNPS_ACCEPT(r2, hi2, a.k2, Aj.w) && ((a.source_mask >> (__float_as_int(Cj.w) & 7)) & 1u)) {
                 npairs++;
                 const float rinv = r2 > 1e-24f ? frsqrt(r2) : 0.0f;
                 const float h1 = frcp(0.5f * (Ai.w + Aj.w));
@@ -236,12 +235,8 @@ __global__ void __launch_bounds__(LIST_NT, 4) k_solid_pass1(const SolidArgs a, c
         a.R2[s] = make_float4(rr[2], rr[3], rr[4], rr[5]);
         a.C3[s].y = (float)p;
     }
-    if (a.pair_counter) {
-        if (ti & PT_GHOST) npairs = 0;   // ghost destinations (ghost_group1) are the owner's pairs
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) npairs += __shfl_xor_sync(FULL, npairs, o);
-        if ((tid & 31) == 0 && npairs) atomicAdd(a.pair_counter, (unsigned long long)npairs);
-    }
+    if (ti & PT_GHOST) npairs = 0;   // ghost destinations (ghost_group1) are the owner's pairs
+    pairs_flush(a, npairs);
 }
 
 // group 2: ContinuityEquation, MomentumEquationWithStress, MonaghanArtificialViscosity, XSPHCorrection
@@ -268,7 +263,7 @@ __global__ void __launch_bounds__(LIST_NT, 4) k_solid_pass2(const SolidArgs a, c
     int cmax = count;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) cmax = max(cmax, __shfl_xor_sync(FULL, cmax, o));
-    const uint32_t *my = lst + ((size_t)(s >> 5) * (size_t)capg) * 32u + (uint32_t)(s & 31);
+    const uint32_t *my = list_slot(lst, capg, s);
     const float hi2 = a.k2 * Ai.w * Ai.w;
     const float wdp = a.wdeltap[ti & 7], nexp = a.nexp[ti & 7];
     const float wdp1 = wdp > 0.f ? frcp(wdp) : 0.f;
@@ -283,11 +278,10 @@ __global__ void __launch_bounds__(LIST_NT, 4) k_solid_pass2(const SolidArgs a, c
         },
         [&](const bool live, const uint32_t e, const Rec &r) {
             const float4 Aj = r.A, Bj = r.B, Cj = r.C, Tj1 = r.T1, Tj2 = r.T2, Tj3 = r.T3;
-            const float4 T = list_cell_offset(e, a.cellx, a.celly, a.cellz);
-            const float xij = Ai.x - Aj.x + T.x, yij = Ai.y - Aj.y + T.y, zij = Ai.z - Aj.z + T.z;
-            const float r2 = xij * xij + yij * yij + zij * zij;
+            float xij, yij, zij;
+            const float r2 = list_dist(e, a.cellx, a.celly, a.cellz, Ai, Aj, xij, yij, zij);
             const int tj = __float_as_int(Cj.w) & 7;
-            if (live && ((r2 < hi2) || (r2 < a.k2 * Aj.w * Aj.w)) && ((a.source_mask >> tj) & 1u)) {
+            if (live && NNPS_ACCEPT(r2, hi2, a.k2, Aj.w) && ((a.source_mask >> tj) & 1u)) {
                 npairs++;
                 const float rinv = r2 > 1e-24f ? frsqrt(r2) : 0.0f;
                 const float hij = 0.5f * (Ai.w + Aj.w);
@@ -337,11 +331,7 @@ __global__ void __launch_bounds__(LIST_NT, 4) k_solid_pass2(const SolidArgs a, c
         a.au[g] = au; a.av[g] = av; a.aw[g] = aw;
         a.ax[g] = ax + Bi.x; a.ay[g] = ay + Bi.y; a.az[g] = az + Bi.z;   // post_loop :297-300
     }
-    if (a.pair_counter) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) npairs += __shfl_xor_sync(FULL, npairs, o);
-        if ((tid & 31) == 0 && npairs) atomicAdd(a.pair_counter, (unsigned long long)npairs);
-    }
+    pairs_flush(a, npairs);
 }
 
 struct StageSolidArgs {

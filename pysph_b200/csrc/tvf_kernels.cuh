@@ -90,7 +90,7 @@ __global__ void __launch_bounds__(LIST_NT, 4) k_tvf_pass1(const TvfArgs a, const
     int cmax = count;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) cmax = max(cmax, __shfl_xor_sync(FULL, cmax, o));
-    const uint32_t *my = lst + ((size_t)(s >> 5) * (size_t)capg) * 32u + (uint32_t)(s & 31);
+    const uint32_t *my = list_slot(lst, capg, s);
     const float hi2 = a.k2 * Ai.w * Ai.w;
     float wsum = 0.f, psum = 0.f, nn = 0.f;
     unsigned npairs = 0;
@@ -104,10 +104,9 @@ __global__ void __launch_bounds__(LIST_NT, 4) k_tvf_pass1(const TvfArgs a, const
         [&](const bool live, const uint32_t e, const Rec &r) {
             const float4 Aj = r.A;
             const float2 Pj = r.P;
-            const float4 T = list_cell_offset(e, a.cellx, a.celly, a.cellz);
-            const float xij = Ai.x - Aj.x + T.x, yij = Ai.y - Aj.y + T.y, zij = Ai.z - Aj.z + T.z;
-            const float r2 = xij * xij + yij * yij + zij * zij;
-            if (live && ((r2 < hi2) || (r2 < a.k2 * Aj.w * Aj.w)) && ((a.src_mask >> (__float_as_int(Pj.y) & 7)) & 1u)) {
+            float xij, yij, zij;
+            const float r2 = list_dist(e, a.cellx, a.celly, a.cellz, Ai, Aj, xij, yij, zij);
+            if (live && NNPS_ACCEPT(r2, hi2, a.k2, Aj.w) && ((a.src_mask >> (__float_as_int(Pj.y) & 7)) & 1u)) {
                 npairs++;
                 const float rij = sqrtf(r2);
                 const float h1 = frcp(0.5f * (Ai.w + Aj.w));
@@ -134,11 +133,7 @@ __global__ void __launch_bounds__(LIST_NT, 4) k_tvf_pass1(const TvfArgs a, const
             a.Dv[s].w = pv;
         }
     }
-    if (a.pair_counter) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) npairs += __shfl_xor_sync(FULL, npairs, o);
-        if ((tid & 31) == 0 && npairs) atomicAdd(a.pair_counter, (unsigned long long)npairs);
-    }
+    pairs_flush(a, npairs);
 }
 
 // group 1, the wall arrays (real=False; wc/edac.py:815-822), after k_tvf_pass1 has put the
@@ -176,7 +171,7 @@ __global__ void __launch_bounds__(LIST_NT, 4) k_tvf_wall(const TvfArgs a, const 
     int cmax = count;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) cmax = max(cmax, __shfl_xor_sync(FULL, cmax, o));
-    const uint32_t *my = lst + ((size_t)(s >> 5) * (size_t)capg) * 32u + (uint32_t)(s & 31);
+    const uint32_t *my = list_slot(lst, capg, s);
     const float hi2 = a.k2 * Ai.w * Ai.w;
     float vsum = 0.f, wsum = 0.f, psum = 0.f, us = 0.f, vs = 0.f, ws = 0.f;
     unsigned npairs = 0;
@@ -189,11 +184,10 @@ __global__ void __launch_bounds__(LIST_NT, 4) k_tvf_wall(const TvfArgs a, const 
         },
         [&](const bool live, const uint32_t e, const Rec &r) {
             const float4 Aj = r.A, Bj = r.B, Cj = r.C;
-            const float4 T = list_cell_offset(e, a.cellx, a.celly, a.cellz);
-            const float xij = Ai.x - Aj.x + T.x, yij = Ai.y - Aj.y + T.y, zij = Ai.z - Aj.z + T.z;
-            const float r2 = xij * xij + yij * yij + zij * zij;
+            float xij, yij, zij;
+            const float r2 = list_dist(e, a.cellx, a.celly, a.cellz, Ai, Aj, xij, yij, zij);
             const int tj = __float_as_int(Cj.w) & 7;
-            if (live && ((r2 < hi2) || (r2 < a.k2 * Aj.w * Aj.w)) && ((a.src_mask >> tj) & 1u)) {
+            if (live && NNPS_ACCEPT(r2, hi2, a.k2, Aj.w) && ((a.src_mask >> tj) & 1u)) {
                 npairs++;
                 const float rij = sqrtf(r2);
                 const float h1 = frcp(0.5f * (Ai.w + Aj.w));
@@ -228,11 +222,7 @@ __global__ void __launch_bounds__(LIST_NT, 4) k_tvf_wall(const TvfArgs a, const 
         float2 *pt = const_cast<float2 *>(a.PT) + s;
         pt->x = pw;
     }
-    if (a.pair_counter) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) npairs += __shfl_xor_sync(FULL, npairs, o);
-        if ((tid & 31) == 0 && npairs) atomicAdd(a.pair_counter, (unsigned long long)npairs);
-    }
+    pairs_flush(a, npairs);
 }
 
 // group 2 (real=True): pressure gradient with the background-pressure term, artificial /
@@ -266,7 +256,7 @@ __global__ void __launch_bounds__(LIST_NT, 6) k_tvf_pass2(const TvfArgs a, const
     int cmax = count;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) cmax = max(cmax, __shfl_xor_sync(FULL, cmax, o));
-    const uint32_t *my = lst + ((size_t)(s >> 5) * (size_t)capg) * 32u + (uint32_t)(s & 31);
+    const uint32_t *my = list_slot(lst, capg, s);
     const float hi2 = a.k2 * Ai.w * Ai.w;
     const float rhoi = Ci.x, pi = Ci.y, pavg = Di.w;
     const float Vi1 = frcp(Ci.z);
@@ -287,12 +277,11 @@ __global__ void __launch_bounds__(LIST_NT, 6) k_tvf_pass2(const TvfArgs a, const
         },
         [&](const bool live, const uint32_t e, const Rec &r) {
             const float4 Aj = r.A, Bj = r.B, Cj = r.C, Dj = r.D;
-            const float4 T = list_cell_offset(e, a.cellx, a.celly, a.cellz);
-            const float xij = Ai.x - Aj.x + T.x, yij = Ai.y - Aj.y + T.y, zij = Ai.z - Aj.z + T.z;
-            const float r2 = xij * xij + yij * yij + zij * zij;
+            float xij, yij, zij;
+            const float r2 = list_dist(e, a.cellx, a.celly, a.cellz, Ai, Aj, xij, yij, zij);
             const int tj = __float_as_int(Cj.w) & 7;
             const bool wall = WALLS && ((a.solid_mask >> tj) & 1u);
-            if (live && ((r2 < hi2) || (r2 < a.k2 * Aj.w * Aj.w)) && (((WALLS ? a.src_mask : a.fluid_mask) >> tj) & 1u)) {
+            if (live && NNPS_ACCEPT(r2, hi2, a.k2, Aj.w) && (((WALLS ? a.src_mask : a.fluid_mask) >> tj) & 1u)) {
                 npairs++;
                 const bool far = r2 > 1e-24f;
                 const float rinv = far ? frsqrt(r2) : 0.0f;
@@ -379,11 +368,7 @@ __global__ void __launch_bounds__(LIST_NT, 6) k_tvf_pass2(const TvfArgs a, const
         a.au[g] = au; a.av[g] = av; a.aw[g] = aw;
         if (a.eqbits & B200SPH_TVF_EDAC) a.ap[g] = ap;
     }
-    if (a.pair_counter) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) npairs += __shfl_xor_sync(FULL, npairs, o);
-        if ((tid & 31) == 0 && npairs) atomicAdd(a.pair_counter, (unsigned long long)npairs);
-    }
+    pairs_flush(a, npairs);
 }
 
 struct StageTvfArgs {
