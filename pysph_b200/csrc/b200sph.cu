@@ -222,6 +222,30 @@ struct PendingEvent {
     int slot;  // 0 nnps, 1 pair, 2 other
 };
 
+// A buffer the context owns: `cap` elements of device memory, or of page-locked host memory
+// (PINNED: cudaMallocHost; MAPPED: cudaHostAlloc with a device alias).  It frees itself, so the
+// context frees every buffer by being deleted; grow() below is the one place that allocates.
+// It reads as the raw pointer (launches, argument structs, copies).
+enum class Mem { DEVICE, PINNED, MAPPED };
+template <class T, Mem M = Mem::DEVICE> struct Buf {
+    T *p = nullptr;
+    size_t cap = 0;
+    Buf() = default;
+    Buf(Buf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr, o.cap = 0; }
+    Buf &operator=(Buf &&o) noexcept { std::swap(p, o.p), std::swap(cap, o.cap); return *this; }
+    ~Buf() { reset(); }
+    cudaError_t reset()
+    {
+        const cudaError_t e = !p ? cudaSuccess : M == Mem::DEVICE ? cudaFree(p) : cudaFreeHost(p);
+        p = nullptr, cap = 0;
+        return e;
+    }
+    operator T *() const { return p; }
+    T *operator->() const { return p; }
+};
+struct PeerBox;
+struct PeerDecision;
+
 struct b200sph_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -239,10 +263,10 @@ struct b200sph_ctx {
     // which by x0 .. rho0 changes when a fused stage 1 takes the initialize by renaming
     // (init_by_rename): read these at enqueue time, and keep no copy of them across a stage
     void *prop[N_PROP_SLOTS] = {nullptr};
-    float4 *Dv = nullptr;               // sorted: (uhat-u, vhat-v, what-w, pavg)
-    float4 *T01 = nullptr, *T2R = nullptr, *R2 = nullptr;   // sorted stress records (with the elastic group)
-    float2 *PT = nullptr;               // sorted: (p, type)
-    uint8_t *ptype = nullptr;
+    Buf<float4> Dv;                     // sorted: (uhat-u, vhat-v, what-w, pavg)
+    Buf<float4> T01, T2R, R2;           // sorted stress records (with the elastic group)
+    Buf<float2> PT;                     // sorted: (p, type)
+    Buf<uint8_t> ptype;
     bool ptype_dirty = true;
 
     int kernel = 0, dim = 3;
@@ -256,8 +280,8 @@ struct b200sph_ctx {
     double mirror_layers = 2.0;
     struct MirrorSeg {
         int arr, axis, side;
-        int64_t count = 0, cap = 0, ghost_first = 0;   // ghost_first: relative to the array's first ghost
-        uint32_t *idx = nullptr;                        // sources, relative to the array's offset
+        int64_t count = 0, ghost_first = 0;             // ghost_first: relative to the array's first ghost
+        Buf<uint32_t> idx;                              // sources, relative to the array's offset
     };
     std::vector<MirrorSeg> mirror_segs;                 // in creation order (corner images read earlier ones)
     bool mirror_built = false;
@@ -270,20 +294,16 @@ struct b200sph_ctx {
     double last_domain_size = 0.0;
 
     // sort / cell list buffers
-    int64_t sort_cap = 0;        // particles
-    int64_t cell_cap = 0;        // cells (+1)
-    uint32_t *key_of = nullptr;  // [pool] cell key per particle
-    uint32_t *off_in = nullptr;  // [pool] arrival rank inside the cell
-    uint32_t *cell_cnt = nullptr;
-    uint32_t *cell_start = nullptr;
-    uint32_t *blk_sums = nullptr;
-    int64_t blk_cap = 0;
-    uint32_t *perm_tmp = nullptr, *perm = nullptr, *skey = nullptr, *rank = nullptr;
-    float4 *A = nullptr, *B = nullptr, *C = nullptr;
-    float4 *AB = nullptr;  // {A, B} interleaved (32 B = one sector per particle) for the list consumer's 256-bit gathers
+    Buf<uint32_t> key_of;        // [pool] cell key per particle
+    Buf<uint32_t> off_in;        // [pool] arrival rank inside the cell
+    Buf<uint32_t> cell_cnt, cell_start;
+    Buf<uint32_t> blk_sums;
+    Buf<uint32_t> perm_tmp, perm, skey, rank;
+    Buf<float4> A, B, C;
+    Buf<float4> AB;  // {A, B} interleaved (32 B = one sector per particle) for the list consumer's 256-bit gathers
     // the 32-byte records of the WCSPH pass (records32): {(x, y, z, p / rho^2), (u, v, w, delta + type)};
     // while rec32 holds, the state records are packed HERE instead of B / C / the B half of AB
-    float4 *R = nullptr;
+    Buf<float4> R;
     bool rec32 = false;
     Rec32Eos rec32_eos = {};    // the EOS the records are packed with
     bool ab_stale = false;      // k_stage_pack wrote the positions into R only (ab_positions restores AB)
@@ -307,10 +327,9 @@ struct b200sph_ctx {
     double S_abs = 0.0;         // absolute skin of the current build
     double cell_int = 1.0;      // internal cell size (cell_size + S)
     GridDev G;                  // frozen device grid of the current build
-    float4 *A0 = nullptr;       // packed positions at build time
-    uint32_t *lst = nullptr;    // transposed lists: [n/32][capg][32]
-    int64_t lst_cap = 0;        // entries allocated
-    uint32_t *cnt = nullptr;    // [n] list length per destination
+    Buf<float4> A0;             // packed positions at build time
+    Buf<uint32_t> lst;          // transposed lists: [n/32][capg][32]
+    Buf<uint32_t> cnt;          // [n] list length per destination
     int capg = 0;               // entries reserved per destination
     bool lists_valid = false;
     bool topo_dirty = true;     // particle set / h pushed: a light update is not enough
@@ -318,7 +337,7 @@ struct b200sph_ctx {
     // deferred drift check (b200sph_nnps_update_deferred / b200sph_nnps_confirm)
     bool defer_check = false;   // the running nnps_update may leave its drift check pending
     bool check_pending = false; // a light update ran on the assumption that the lists are valid
-    unsigned *drift_host = nullptr;
+    Buf<unsigned, Mem::PINNED> drift_host;
     cudaEvent_t drift_evt = nullptr;
     int64_t n_deferred_failed = 0;
     // proactive rebuild: the used-up fraction of the skin at the last two confirmed deferred
@@ -328,13 +347,12 @@ struct b200sph_ctx {
     bool proactive = true;      // env B200SPH_PROACTIVE=0
     int64_t n_proactive = 0;
     // device-resident time control block: [0] dt, [1] t, [2] proposed dt, [3] h_minimum
-    double *tc = nullptr;
-    bool tc_owned = false;
-    double *tc_host = nullptr;          // pinned: 2 snapshot slots x 2 doubles
+    double *tc = nullptr;               // tc_own, or the caller's block (b200sph_time_control)
+    Buf<double> tc_own;
+    Buf<double, Mem::PINNED> tc_host;   // 2 snapshot slots x 2 doubles
     double t_final = INFINITY, t_eps = 0.0;  // b200sph_time_final: the last dt lands on t_final
     // asynchronous output snapshot (b200sph_snapshot_*): one in flight
-    double *snap_buf = nullptr;         // device staging, 8-byte slots
-    int64_t snap_cap = 0;               // in doubles
+    Buf<double> snap_buf;               // device staging, 8-byte slots
     std::vector<int64_t> snap_off, snap_len;   // per segment: offset (doubles) / elements
     std::vector<int> snap_u32;          // per segment: 1 = 4-byte integers
     cudaStream_t snap_stream = nullptr; // the D2H copies run here, beside the time loop
@@ -342,22 +360,21 @@ struct b200sph_ctx {
     std::atomic<bool> snap_open{false};   // taken by the time loop, released by the output thread
     cudaEvent_t tc_evt[2] = {nullptr, nullptr};
     bool h_dirty = true;        // h changed since the last update_domain reduction
-    unsigned *red_u32 = nullptr, *red_u32_host = nullptr;
+    Buf<unsigned> red_u32;
+    Buf<unsigned, Mem::PINNED> red_u32_host;
     int64_t n_full_builds = 0, n_light_updates = 0, n_list_builds = 0;
 
     // scratch
-    long long *red = nullptr;     // 16 ordered-int64 slots
-    long long *red_host = nullptr;  // pinned
-    unsigned long long *counter = nullptr;  // pair counter + misc
-    unsigned long long *counter_host = nullptr;
-    double *stage_buf = nullptr;  // host<->device staging for f32 props
-    int64_t stage_cap = 0;
-    uint32_t *flag_a = nullptr, *flag_b = nullptr;  // [pool+1] scan scratch
-    int64_t flag_cap = 0;
+    Buf<long long> red;           // 16 ordered-int64 slots
+    Buf<long long, Mem::PINNED> red_host;
+    Buf<unsigned long long> counter;  // pair counter + misc
+    Buf<unsigned long long, Mem::PINNED> counter_host;
+    Buf<double> stage_buf;        // host<->device staging for f32 props
+    Buf<uint32_t> flag_a, flag_b; // [pool+1] scan scratch
 
     // persistent halo: pool-relative indices of the real particles sent to neighbour `slot`
-    uint32_t *halo_idx[B200SPH_MAX_ARRAYS][2] = {{nullptr}};
-    int64_t halo_cnt[B200SPH_MAX_ARRAYS][2] = {{0}}, halo_cap[B200SPH_MAX_ARRAYS][2] = {{0}};
+    Buf<uint32_t> halo_idx[B200SPH_MAX_ARRAYS][2];
+    int64_t halo_cnt[B200SPH_MAX_ARRAYS][2] = {{0}};
 
     EosTab eos_pending;
     bool eos_any = false;
@@ -367,13 +384,14 @@ struct b200sph_ctx {
     bool eos_pool_any = false;
     // ---- peer protocol (b200sph_peer_*) + interior / boundary split of the list consumer --
     int peer_rank = -1, peer_world = 0;
-    struct PeerBox *peer_box = nullptr;          // this rank's mailbox
-    struct PeerBox *peer_boxes[B200SPH_MAX_RANKS] = {nullptr};   // every rank's (own: the local one)
+    Buf<PeerBox> peer_box;                       // this rank's mailbox
+    PeerBox *peer_boxes[B200SPH_MAX_RANKS] = {nullptr};   // every rank's (own: the local one)
     bool peer_connected = false;
     unsigned long long peer_epoch = 0, peer_dt_epoch = 0;
-    unsigned *peer_done = nullptr;               // "blocks finished" counters of k_peer_push, one per direction
-    double *peer_dec_dev = nullptr;
-    struct PeerDecision *peer_dec_host = nullptr, *peer_dec_hostdev = nullptr;   // pinned + its device alias
+    Buf<unsigned> peer_done;                     // "blocks finished" counters of k_peer_push, one per direction
+    Buf<double> peer_dec_dev;
+    Buf<PeerDecision, Mem::MAPPED> peer_dec_host;
+    PeerDecision *peer_dec_hostdev = nullptr;    // the device alias of peer_dec_host
     cudaStream_t comm_stream = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     // profiling of the overlapped evaluation (b200sph_set_profiling != 0): per pair pass an event
@@ -388,19 +406,16 @@ struct b200sph_ctx {
     // generic-equation fallback: run-time compiled modules
     std::vector<void *> gen_modules;             // CUmodule (or, emulated, a dlopen handle)
     // density_filter: its records, [2 n_sorted] (allocated on first use)
-    float4 *dfilter_F = nullptr;
-    size_t dfilter_cap = 0;
+    Buf<float4> dfilter_F;
     // interpolation (b200sph_probe_*, b200sph_interpolate): the probe sets by id (xyz: 3 n doubles,
     // null once released), the records [2 n_sorted] and order1's rho [n_sorted], the reach
     // reduction and the results (allocated on first use)
-    struct ProbeSet { double *xyz = nullptr; int64_t n = 0; double h = 0.0; };
+    struct ProbeSet { Buf<double> xyz; int64_t n = 0; double h = 0.0; };
     std::vector<ProbeSet> probes;
-    float4 *interp_Q = nullptr;
-    float *interp_rho = nullptr;
-    size_t interp_cap = 0;
-    unsigned *interp_red = nullptr;
-    double *interp_out = nullptr;
-    size_t interp_out_cap = 0;
+    Buf<float4> interp_Q;
+    Buf<float> interp_rho;
+    Buf<unsigned> interp_red;
+    Buf<double> interp_out;
     // Group(start_idx, stop_idx): one-shot destination ranges of the next pair pass
     int64_t dst_lo[B200SPH_MAX_ARRAYS] = {0}, dst_hi[B200SPH_MAX_ARRAYS] = {0};
     bool dst_ranged = false;
@@ -408,11 +423,11 @@ struct b200sph_ctx {
     // peer_publish / peer_send / peer_recv only RECORD: the launches are merged into one
     // k_peer_push (at peer_reduce) and one k_peer_pull (at peer_end)
     struct PeerPending *pend = nullptr;
-    uint8_t *sflag = nullptr;                    // [sorted] 1 = ghost
-    uint8_t *stype = nullptr;                    // [sorted] particle type byte (array id | ghost bit), written by k_pack_pos
+    Buf<uint8_t> sflag;                          // [sorted] 1 = ghost
+    Buf<uint8_t> stype;                          // [sorted] particle type byte (array id | ghost bit), written by k_pack_pos
     unsigned long long list_mask[B200SPH_MAX_ARRAYS] = {0};   // the equation mask the current lists were filtered with
-    uint32_t *chunk_boundary = nullptr, *chunk_interior = nullptr;
-    int64_t n_chunk_boundary = 0, n_chunk_interior = 0, chunk_cap = 0;
+    Buf<uint32_t> chunk_boundary, chunk_interior;
+    int64_t n_chunk_boundary = 0, n_chunk_interior = 0;
     bool chunks_valid = false;
     int64_t n_overlapped = 0;
     // ---- fused stage kernel (k_stage_pack) bookkeeping ---------------------------------
@@ -555,6 +570,27 @@ static int set_err(b200sph_ctx *c, const char *fmt, ...)
             return set_err(ctx, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_e), \
                            __FILE__, __LINE__);                                     \
     } while (0)
+
+// b holds at least `need` elements afterwards: a smaller buffer is freed and `reserve` (>= need)
+// elements are allocated -- freed first, so that the old and the new one never take the card
+// together.  Contents are not kept.  On failure b is left empty.
+template <class T, Mem M> static int grow(b200sph_ctx *ctx, Buf<T, M> &b, size_t need, size_t reserve)
+{
+    if (need <= b.cap) return 0;
+    cudaError_t e = b.reset();
+    const size_t bytes = sizeof(T) * reserve;
+    if (e == cudaSuccess)
+        e = M == Mem::DEVICE ? cudaMalloc((void **)&b.p, bytes)
+          : M == Mem::PINNED ? cudaMallocHost((void **)&b.p, bytes)
+                             : cudaHostAlloc((void **)&b.p, bytes, cudaHostAllocMapped);
+    if (e != cudaSuccess) {
+        b.p = nullptr;
+        return set_err(ctx, "cannot allocate %.1f MB of %s memory: %s", 1e-6 * (double)bytes,
+                       M == Mem::DEVICE ? "device" : "pinned host", cudaGetErrorString(e));
+    }
+    b.cap = reserve;
+    return 0;
+}
 
 #define LAUNCH_CHECK()                                                              \
     do {                                                                            \
@@ -729,14 +765,6 @@ static int pool_layout(b200sph_ctx *ctx, const int64_t *new_cap)
         }
         ctx->prop[p] = nw;
     }
-    if (elastic_allocated(ctx)) {
-        for (float4 **r : {&ctx->T01, &ctx->T2R, &ctx->R2}) {
-            if (*r) CU(cudaFree(*r));
-            CU(cudaMalloc((void **)r, 16 * (size_t)alloc));
-        }
-    }
-    if (ctx->ptype) CU(cudaFree(ctx->ptype));
-    CU(cudaMalloc((void **)&ctx->ptype, (size_t)alloc));
     for (int a = 0; a < ctx->narr; a++) {
         ctx->arr[a].off = new_off[a];
         ctx->arr[a].cap = new_cap[a];
@@ -744,45 +772,24 @@ static int pool_layout(b200sph_ctx *ctx, const int64_t *new_cap)
     ctx->pool_cap = alloc;
     ctx->pool_end = total;
     pool_moved(ctx);
-    // per-particle work buffers
-    if (ctx->key_of) cudaFree(ctx->key_of);
-    if (ctx->off_in) cudaFree(ctx->off_in);
-    if (ctx->perm_tmp) cudaFree(ctx->perm_tmp);
-    if (ctx->perm) cudaFree(ctx->perm);
-    if (ctx->skey) cudaFree(ctx->skey);
-    if (ctx->rank) cudaFree(ctx->rank);
-    if (ctx->A) cudaFree(ctx->A);
-    if (ctx->B) cudaFree(ctx->B);
-    if (ctx->C) cudaFree(ctx->C);
-    if (ctx->AB) cudaFree(ctx->AB);
-    if (ctx->R) cudaFree(ctx->R);
-    if (ctx->A0) cudaFree(ctx->A0);
-    if (ctx->Dv) cudaFree(ctx->Dv);
-    if (ctx->PT) cudaFree(ctx->PT);
-    if (ctx->cnt) cudaFree(ctx->cnt);
-    if (ctx->flag_a) cudaFree(ctx->flag_a);
-    if (ctx->flag_b) cudaFree(ctx->flag_b);
-    CU(cudaMalloc((void **)&ctx->key_of, 4 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->off_in, 4 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->perm_tmp, 4 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->perm, 4 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->skey, 4 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->rank, 4 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->A, 16 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->B, 16 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->C, 16 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->AB, 32 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->R, 32 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->A0, 16 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->Dv, 16 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->PT, 8 * (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->cnt, 4 * (size_t)alloc));
-    if (ctx->stype) cudaFree(ctx->stype);
-    CU(cudaMalloc((void **)&ctx->stype, (size_t)alloc));
-    CU(cudaMalloc((void **)&ctx->flag_a, 4 * (size_t)(alloc + 1)));
-    CU(cudaMalloc((void **)&ctx->flag_b, 4 * (size_t)(alloc + 1)));
-    ctx->flag_cap = alloc + 1;
-    ctx->sort_cap = alloc;
+    // per-particle work buffers (their contents are stale now): AB and R hold two float4 per
+    // particle, the scan scratch flag_a / flag_b one entry more
+    const size_t n = (size_t)alloc;
+    int rc;
+    for (Buf<uint32_t> *b : {&ctx->key_of, &ctx->off_in, &ctx->perm_tmp, &ctx->perm, &ctx->skey, &ctx->rank, &ctx->cnt})
+        if ((rc = grow(ctx, *b, n, n))) return rc;
+    for (Buf<uint32_t> *b : {&ctx->flag_a, &ctx->flag_b})
+        if ((rc = grow(ctx, *b, n + 1, n + 1))) return rc;
+    for (Buf<float4> *b : {&ctx->A, &ctx->B, &ctx->C, &ctx->A0, &ctx->Dv})
+        if ((rc = grow(ctx, *b, n, n))) return rc;
+    for (Buf<float4> *b : {&ctx->AB, &ctx->R})
+        if ((rc = grow(ctx, *b, 2 * n, 2 * n))) return rc;
+    for (Buf<uint8_t> *b : {&ctx->ptype, &ctx->stype})
+        if ((rc = grow(ctx, *b, n, n))) return rc;
+    if ((rc = grow(ctx, ctx->PT, n, n))) return rc;
+    if (elastic_allocated(ctx))
+        for (Buf<float4> *b : {&ctx->T01, &ctx->T2R, &ctx->R2})
+            if ((rc = grow(ctx, *b, n, n))) return rc;
     return 0;
 }
 
@@ -847,11 +854,7 @@ static int ensure_pool(b200sph_ctx *ctx, bool join = true, bool keep_init = fals
 static int device_scan(b200sph_ctx *ctx, const uint32_t *in, uint32_t *out, int64_t n)
 {
     const int64_t nb = cdiv(n, SCAN_TILE);
-    if (nb > ctx->blk_cap) {
-        if (ctx->blk_sums) CU(cudaFree(ctx->blk_sums));
-        CU(cudaMalloc((void **)&ctx->blk_sums, 4 * (size_t)(nb + 1024)));
-        ctx->blk_cap = nb + 1024;
-    }
+    if (int rc = grow(ctx, ctx->blk_sums, nb, nb + 1024)) return rc;
     k_scan_tiles<<<(unsigned)nb, SCAN_THREADS, 0, ctx->stream>>>(in, out, n, ctx->blk_sums);
     LAUNCH_CHECK();
     if (nb > 1) {
@@ -1063,17 +1066,17 @@ int b200sph_create(int device, b200sph_ctx **out)
     if (const char *e = getenv("B200SPH_SKIN_ADAPT")) ctx->skin_adapt = atoi(e) != 0;
     if (const char *e = getenv("B200SPH_RECORDS")) ctx->rec48_forced = atoi(e) == 48;
     ctx->skin_min = std::min(ctx->skin_min, ctx->skin_max);
-    CU(cudaMalloc((void **)&ctx->red_u32, 4 * sizeof(unsigned)));
-    CU(cudaMallocHost((void **)&ctx->red_u32_host, 4 * sizeof(unsigned)));
-    CU(cudaMallocHost((void **)&ctx->drift_host, 4 * sizeof(unsigned)));
+    int rc;
+    if ((rc = grow(ctx, ctx->red_u32, 4, 4)) || (rc = grow(ctx, ctx->red_u32_host, 4, 4)) ||
+        (rc = grow(ctx, ctx->drift_host, 4, 4)) || (rc = grow(ctx, ctx->red, 16, 16)) ||
+        (rc = grow(ctx, ctx->red_host, 16, 16)) || (rc = grow(ctx, ctx->counter, 8, 8)) ||
+        (rc = grow(ctx, ctx->counter_host, 8, 8)))
+        return rc;
     CU(cudaEventCreateWithFlags(&ctx->drift_evt, cudaEventDisableTiming));
-    CU(cudaMalloc((void **)&ctx->red, 16 * sizeof(long long)));
-    CU(cudaMallocHost((void **)&ctx->red_host, 16 * sizeof(long long)));
-    CU(cudaMalloc((void **)&ctx->counter, 8 * sizeof(unsigned long long)));
-    CU(cudaMallocHost((void **)&ctx->counter_host, 8 * sizeof(unsigned long long)));
     return 0;
 }
 
+// the buffers free themselves (Buf) when ctx is deleted, after the streams have drained
 int b200sph_destroy(b200sph_ctx *ctx)
 {
     if (!ctx) return 0;
@@ -1081,22 +1084,6 @@ int b200sph_destroy(b200sph_ctx *ctx)
     cudaStreamSynchronize(ctx->stream);
     for (void *b : ctx->prop) cudaFree(b);
     generic_unload_all(ctx);
-    cudaFree(ctx->Dv); cudaFree(ctx->PT); cudaFree(ctx->dfilter_F);
-    for (auto &ps : ctx->probes) cudaFree(ps.xyz);
-    cudaFree(ctx->interp_Q); cudaFree(ctx->interp_rho); cudaFree(ctx->interp_red); cudaFree(ctx->interp_out);
-    for (auto &sg : ctx->mirror_segs) cudaFree(sg.idx);
-    cudaFree(ctx->T01); cudaFree(ctx->T2R); cudaFree(ctx->R2);
-    cudaFree(ctx->ptype);
-    cudaFree(ctx->key_of); cudaFree(ctx->off_in); cudaFree(ctx->cell_cnt); cudaFree(ctx->cell_start);
-    cudaFree(ctx->blk_sums); cudaFree(ctx->perm_tmp); cudaFree(ctx->perm); cudaFree(ctx->skey);
-    cudaFree(ctx->rank); cudaFree(ctx->A); cudaFree(ctx->B); cudaFree(ctx->C); cudaFree(ctx->AB); cudaFree(ctx->R);
-    cudaFree(ctx->red); cudaFreeHost(ctx->red_host); cudaFree(ctx->counter);
-    cudaFreeHost(ctx->counter_host); cudaFree(ctx->stage_buf); cudaFree(ctx->flag_a);
-    cudaFree(ctx->flag_b); cudaFree(ctx->A0); cudaFree(ctx->lst); cudaFree(ctx->cnt);
-    cudaFree(ctx->red_u32); cudaFreeHost(ctx->red_u32_host);
-    cudaFreeHost(ctx->drift_host);
-    if (ctx->tc_owned) cudaFree(ctx->tc);
-    if (ctx->tc_host) cudaFreeHost(ctx->tc_host);
     for (int i = 0; i < 2; i++)
         if (ctx->tc_evt[i]) cudaEventDestroy(ctx->tc_evt[i]);
     if (ctx->drift_evt) cudaEventDestroy(ctx->drift_evt);
@@ -1105,11 +1092,8 @@ int b200sph_destroy(b200sph_ctx *ctx)
     if (ctx->snap_stream) { cudaStreamSynchronize(ctx->snap_stream); cudaStreamDestroy(ctx->snap_stream); }
     if (ctx->snap_ready) cudaEventDestroy(ctx->snap_ready);
     if (ctx->snap_done) cudaEventDestroy(ctx->snap_done);
-    cudaFree(ctx->snap_buf);
     for (int r = 0; r < ctx->peer_world; r++)
         if (r != ctx->peer_rank && ctx->peer_boxes[r]) cudaIpcCloseMemHandle(ctx->peer_boxes[r]);
-    cudaFree(ctx->peer_box); cudaFree(ctx->peer_done); cudaFree(ctx->peer_dec_dev);
-    if (ctx->peer_dec_host) cudaFreeHost(ctx->peer_dec_host);
     if (ctx->comm_stream) { cudaStreamSynchronize(ctx->comm_stream); cudaStreamDestroy(ctx->comm_stream); }
     if (ctx->red_stream) { cudaStreamSynchronize(ctx->red_stream); cudaStreamDestroy(ctx->red_stream); }
     if (ctx->ev_pushed) cudaEventDestroy(ctx->ev_pushed);
@@ -1117,7 +1101,6 @@ int b200sph_destroy(b200sph_ctx *ctx)
     free_peer_pending(ctx);
     if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
     if (ctx->ev_join) cudaEventDestroy(ctx->ev_join);
-    cudaFree(ctx->sflag); cudaFree(ctx->stype); cudaFree(ctx->chunk_boundary); cudaFree(ctx->chunk_interior);
     if (ctx->own_stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
     return 0;
@@ -1217,15 +1200,7 @@ static int check_range(b200sph_ctx *ctx, int arr, int64_t start, int64_t count)
     return 0;
 }
 
-static int ensure_stage(b200sph_ctx *ctx, int64_t count)
-{
-    if (count > ctx->stage_cap) {
-        if (ctx->stage_buf) CU(cudaFree(ctx->stage_buf));
-        CU(cudaMalloc((void **)&ctx->stage_buf, 8 * (size_t)(count + 1024)));
-        ctx->stage_cap = count + 1024;
-    }
-    return 0;
-}
+static int ensure_stage(b200sph_ctx *ctx, int64_t count) { return grow(ctx, ctx->stage_buf, count, count + 1024); }
 
 // a named elastic-dynamics or user property: allocated (zeroed) the first time anything names it,
 // the elastic-dynamics properties as one group with their stress records
@@ -1241,7 +1216,8 @@ static int ensure_prop(b200sph_ctx *ctx, int prop)
         CU(cudaMemsetAsync(ctx->prop[p], 0, esz * alloc, ctx->stream));
     }
     if (g == GROUP_ELASTIC)
-        for (float4 **r : {&ctx->T01, &ctx->T2R, &ctx->R2}) CU(cudaMalloc((void **)r, 16 * alloc));
+        for (Buf<float4> *r : {&ctx->T01, &ctx->T2R, &ctx->R2})
+            if (int rc = grow(ctx, *r, alloc, alloc)) return rc;
     return 0;
 }
 
@@ -1374,11 +1350,7 @@ int b200sph_snapshot_take(b200sph_ctx *ctx, int nseg, const int *arr, const int 
         } else if ((rc = check_range(ctx, arr[i], 0, count[i]))) return rc;
         total += std::max<int64_t>(count[i], 1);
     }
-    if (total > ctx->snap_cap) {
-        if (ctx->snap_buf) CU(cudaFree(ctx->snap_buf));
-        CU(cudaMalloc((void **)&ctx->snap_buf, 8 * (size_t)(total + total / 8 + 1024)));
-        ctx->snap_cap = total + total / 8 + 1024;
-    }
+    if ((rc = grow(ctx, ctx->snap_buf, total, total + total / 8 + 1024))) return rc;
     ctx->snap_off.assign(nseg, 0), ctx->snap_len.assign(nseg, 0), ctx->snap_u32.assign(nseg, 0);
     int64_t at = 0;
     for (int i = 0; i < nseg; i++) {
@@ -1843,14 +1815,8 @@ int b200sph_nnps_update(b200sph_ctx *ctx)
         }
     }
 
-    if (ncells + 2 > ctx->cell_cap) {
-        if (ctx->cell_cnt) CU(cudaFree(ctx->cell_cnt));
-        if (ctx->cell_start) CU(cudaFree(ctx->cell_start));
-        const int64_t cap = ncells + ncells / 2 + 1024;
-        CU(cudaMalloc((void **)&ctx->cell_cnt, 4 * (size_t)cap));
-        CU(cudaMalloc((void **)&ctx->cell_start, 4 * (size_t)cap));
-        ctx->cell_cap = cap;
-    }
+    for (Buf<uint32_t> *b : {&ctx->cell_cnt, &ctx->cell_start})
+        if ((rc = grow(ctx, *b, ncells + 2, ncells + ncells / 2 + 1024))) return rc;
     GridDev &G = ctx->G;
     for (int d = 0; d < 3; d++) {
         G.xmin[d] = mn[d];
@@ -1900,18 +1866,13 @@ static int split_chunks(b200sph_ctx *ctx)
     int64_t nghost = 0;
     for (int a = 0; a < ctx->narr; a++) nghost += ctx->arr[a].n - ctx->arr[a].n_real;
     const int64_t n = ctx->n_sorted, nchunks = cdiv(n, LIST_NT);
-    if (nghost == 0 || n <= 0 || nchunks + 1 > ctx->flag_cap) return 0;
-    if (nchunks > ctx->chunk_cap) {
-        if (ctx->chunk_boundary) CU(cudaFree(ctx->chunk_boundary));
-        if (ctx->chunk_interior) CU(cudaFree(ctx->chunk_interior));
-        if (ctx->sflag) CU(cudaFree(ctx->sflag));
-        ctx->chunk_cap = nchunks + nchunks / 4 + 64;
-        CU(cudaMalloc((void **)&ctx->chunk_boundary, 4 * (size_t)ctx->chunk_cap));
-        CU(cudaMalloc((void **)&ctx->chunk_interior, 4 * (size_t)ctx->chunk_cap));
-        CU(cudaMalloc((void **)&ctx->sflag, (size_t)ctx->chunk_cap * LIST_NT));
-    }
-    int rc = refresh_ptype(ctx);
-    if (rc) return rc;
+    if (nghost == 0 || n <= 0 || (size_t)nchunks + 1 > ctx->flag_a.cap) return 0;
+    const int64_t reserve = nchunks + nchunks / 4 + 64;
+    int rc;
+    for (Buf<uint32_t> *b : {&ctx->chunk_boundary, &ctx->chunk_interior})
+        if ((rc = grow(ctx, *b, nchunks, reserve))) return rc;
+    if ((rc = grow(ctx, ctx->sflag, nchunks * LIST_NT, reserve * LIST_NT))) return rc;
+    if ((rc = refresh_ptype(ctx))) return rc;
     k_sorted_ghost_flag<<<(unsigned)cdiv(n, 256), 256, 0, ctx->stream>>>(ctx->ptype, ctx->perm, n, ctx->sflag);
     LAUNCH_CHECK();
     k_chunk_classify<<<(unsigned)nchunks, LIST_NT, 0, ctx->stream>>>(ctx->cnt, ctx->lst, ctx->capg, ctx->sflag, n, ctx->flag_a);
@@ -1972,16 +1933,9 @@ static int build_lists(b200sph_ctx *ctx, const unsigned long long *want)
         const bool count_only = ctx->capg == 0;
         if (!count_only) {
             const int64_t need = nblk * ctx->capg * 32;
-            if (need > ctx->lst_cap) {
-                if (ctx->lst) CU(cudaFree(ctx->lst));
-                ctx->lst = nullptr;
-                const int64_t cap = need + need / 8;
-                cudaError_t e = cudaMalloc((void **)&ctx->lst, 4 * (size_t)cap);
-                if (e != cudaSuccess) return set_err(ctx, "cannot allocate %.1f GB of neighbour lists: %s", 4e-9 * cap, cudaGetErrorString(e));
-                ctx->lst_cap = cap;
-            }
+            if (int rc = grow(ctx, ctx->lst, need, need + need / 8)) return rc;
         }
-        la.lst = count_only ? nullptr : ctx->lst;
+        la.lst = count_only ? nullptr : ctx->lst.p;
         la.capg = ctx->capg;
         CU(cudaMemsetAsync(ctx->red_u32 + 2, 0, sizeof(unsigned), ctx->stream));
         if (per) k_list_build<true><<<nb, LB_WARPS * 32, 0, ctx->stream>>>(la);
@@ -2116,14 +2070,12 @@ int64_t b200sph_get_neighbors(b200sph_ctx *ctx, int dst_arr, int src_arr, int64_
     CU(cudaMemcpyAsync(&s32, ctx->rank + ctx->arr[dst_arr].off + d_idx, 4, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
     const int64_t dcap = std::max<int64_t>(cap, 1);
-    uint32_t *dout = nullptr;
-    CU(cudaMalloc((void **)&dout, 4 * (size_t)dcap));
+    Buf<uint32_t> dout;
+    if ((rc = grow(ctx, dout, dcap, dcap))) return rc;
     k_neighbors<<<1, 32, 0, ctx->stream>>>(ctx->AB, ctx->C, ctx->cell_start, ctx->skey, ctx->perm, (long long)s32, src_arr,
                                            (long long)ctx->arr[src_arr].off, ctx->G, (float)(ctx->radius_scale * ctx->radius_scale),
                                            dout, cap, ctx->counter + 1);
-    ctx->stats.kernel_launches++;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { cudaFree(dout); return set_err(ctx, "k_neighbors launch failed: %s", cudaGetErrorString(e)); }
+    LAUNCH_CHECK();
     CU(cudaMemcpyAsync(ctx->counter_host + 1, ctx->counter + 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
     const int64_t n = (int64_t)ctx->counter_host[1];
@@ -2132,7 +2084,6 @@ int64_t b200sph_get_neighbors(b200sph_ctx *ctx, int dst_arr, int src_arr, int64_
         CU(cudaMemcpy(out, dout, 4 * (size_t)ncopy, cudaMemcpyDeviceToHost));
         std::sort(out, out + ncopy);
     }
-    cudaFree(dout);
     return n;
 }
 
@@ -2368,12 +2319,7 @@ int b200sph_density_filter(b200sph_ctx *ctx, uint32_t array_mask, int mode, int 
         for (int a = 0; a < ctx->narr; a++)
             if ((array_mask >> a) & 1u) want[a] |= 0xFFull << (8 * a);
         if ((rc = prepare_lists(ctx, want, "density_filter: the neighbour lists cannot index the particles"))) return rc;
-        if ((size_t)ctx->n_sorted > ctx->dfilter_cap) {
-            if (ctx->dfilter_F) CU(cudaFree(ctx->dfilter_F));
-            ctx->dfilter_F = nullptr;
-            CU(cudaMalloc((void **)&ctx->dfilter_F, 2 * sizeof(float4) * (size_t)ctx->n_sorted));
-            ctx->dfilter_cap = (size_t)ctx->n_sorted;
-        }
+        if ((rc = grow(ctx, ctx->dfilter_F, 2 * ctx->n_sorted, 2 * ctx->n_sorted))) return rc;
         PhaseTimer pt(ctx, 1);
         DensityFilterArgs fa;
         memset(&fa, 0, sizeof(fa));
@@ -2417,17 +2363,17 @@ int b200sph_probe_create(b200sph_ctx *ctx, int64_t n, const double *x, const dou
     ps.n = n;
     ps.h = h;
     if (n > 0) {
-        CU(cudaMalloc((void **)&ps.xyz, 24 * (size_t)n));
+        if (int rc = grow(ctx, ps.xyz, 3 * n, 3 * n)) return rc;
         for (int d = 0; d < 3; d++)
             CU(cudaMemcpyAsync(ps.xyz + d * n, d == 0 ? x : (d == 1 ? y : z), 8 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));
     }
     for (size_t i = 0; i < ctx->probes.size(); i++)
         if (ctx->probes[i].n < 0) {
-            ctx->probes[i] = ps;
+            ctx->probes[i] = std::move(ps);
             return (int)i;
         }
-    ctx->probes.push_back(ps);
+    ctx->probes.push_back(std::move(ps));
     return (int)ctx->probes.size() - 1;
 }
 
@@ -2436,8 +2382,7 @@ int b200sph_probe_release(b200sph_ctx *ctx, int id)
     if (id < 0 || id >= (int)ctx->probes.size() || ctx->probes[id].n < 0) return set_err(ctx, "probe_release: no probe set %d", id);
     CU(cudaSetDevice(ctx->device));
     CU(cudaStreamSynchronize(ctx->stream));
-    if (ctx->probes[id].xyz) CU(cudaFree(ctx->probes[id].xyz));
-    ctx->probes[id] = b200sph_ctx::ProbeSet();
+    CU(ctx->probes[id].xyz.reset());
     ctx->probes[id].n = -1;   // a free slot
     return 0;
 }
@@ -2494,21 +2439,10 @@ int b200sph_interpolate(b200sph_ctx *ctx, int id, int method, int kernel, int di
         return 0;
     }
     if ((rc = eos_flush(ctx))) return rc;
-    if ((size_t)ctx->n_sorted > ctx->interp_cap) {
-        if (ctx->interp_Q) CU(cudaFree(ctx->interp_Q));
-        if (ctx->interp_rho) CU(cudaFree(ctx->interp_rho));
-        ctx->interp_Q = nullptr, ctx->interp_rho = nullptr;
-        CU(cudaMalloc((void **)&ctx->interp_Q, 2 * sizeof(float4) * (size_t)ctx->n_sorted));
-        CU(cudaMalloc((void **)&ctx->interp_rho, sizeof(float) * (size_t)ctx->n_sorted));
-        ctx->interp_cap = (size_t)ctx->n_sorted;
-    }
-    if (!ctx->interp_red) CU(cudaMalloc((void **)&ctx->interp_red, 8 * sizeof(unsigned)));
-    if (nout > ctx->interp_out_cap) {
-        if (ctx->interp_out) CU(cudaFree(ctx->interp_out));
-        ctx->interp_out = nullptr;
-        CU(cudaMalloc((void **)&ctx->interp_out, 8 * nout));
-        ctx->interp_out_cap = nout;
-    }
+    const size_t ns = (size_t)ctx->n_sorted;
+    if ((rc = grow(ctx, ctx->interp_Q, 2 * ns, 2 * ns)) || (rc = grow(ctx, ctx->interp_rho, ns, ns)) ||
+        (rc = grow(ctx, ctx->interp_red, 8, 8)) || (rc = grow(ctx, ctx->interp_out, nout, nout)))
+        return rc;
     {
         PhaseTimer pt(ctx, 2);
         ia.x = f64_ptr(ctx, B200SPH_X); ia.y = f64_ptr(ctx, B200SPH_Y); ia.z = f64_ptr(ctx, B200SPH_Z);
@@ -2754,7 +2688,7 @@ int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_
         // slots the interior CTAs free, and there is one tail instead of two.  The main
         // stream joins when the next entry point needs the results (sync_comm).
         for (int phase = 0; phase < (overlap ? 2 : 1); phase++) {
-            const uint32_t *ids = !overlap ? nullptr : (phase == 0 ? ctx->chunk_interior : ctx->chunk_boundary);
+            const uint32_t *ids = !overlap ? nullptr : (phase == 0 ? ctx->chunk_interior.p : ctx->chunk_boundary.p);
             const unsigned nb = (unsigned)(!overlap ? cdiv(ctx->n_sorted, LIST_NT) : (phase == 0 ? ctx->n_chunk_interior : ctx->n_chunk_boundary));
             cudaStream_t lst_stream = ctx->stream;
             if (phase == 1) {
@@ -3039,8 +2973,8 @@ int b200sph_stage_edac_dev(b200sph_ctx *ctx, int arr, int which) { return stage_
 static int ensure_tc(b200sph_ctx *ctx)
 {
     if (ctx->tc) return 0;
-    CU(cudaMalloc((void **)&ctx->tc, 8 * sizeof(double)));
-    ctx->tc_owned = true;
+    if (int rc = grow(ctx, ctx->tc_own, 8, 8)) return rc;
+    ctx->tc = ctx->tc_own;
     const double init[8] = {0.0, 0.0, 1e20, -1.0, 0.0, 0.0, 0.0, 0.0};
     CU(cudaMemcpy(ctx->tc, init, sizeof(init), cudaMemcpyHostToDevice));
     return 0;
@@ -3091,7 +3025,7 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
         q.p = f32_ptr(ctx, B200SPH_P); q.cs = f32_ptr(ctx, B200SPH_CS);
         q.rank = ctx->rank; q.key_of = ctx->key_of;
         q.A0 = ctx->A0; q.AB = ctx->AB; q.C = ctx->C;
-        q.R = ctx->rec32 ? ctx->R : nullptr;   // the layout the last pair pass read
+        q.R = ctx->rec32 ? ctx->R.p : nullptr;   // the layout the last pair pass read
         if (q.R && ctx->hm_known && !std::isnan(ctx->h_uniform)) {   // 8 B per particle less to read
             q.h = nullptr;
             q.h_uniform = ctx->h_uniform;
@@ -3151,15 +3085,14 @@ int b200sph_time_control(b200sph_ctx *ctx, double *external_block8, double **dev
 {
     CU(cudaSetDevice(ctx->device));
     if (external_block8) {
-        if (ctx->tc_owned) CU(cudaFree(ctx->tc));
+        CU(ctx->tc_own.reset());
         ctx->tc = external_block8;
-        ctx->tc_owned = false;
         const double init[8] = {0.0, 0.0, 1e20, -1.0, 0.0, 0.0, 0.0, 0.0};
         CU(cudaMemcpyAsync(ctx->tc, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));
     } else if (int rc = ensure_tc(ctx)) return rc;
     if (!ctx->tc_host) {
-        CU(cudaMallocHost((void **)&ctx->tc_host, 4 * sizeof(double)));
+        if (int rc = grow(ctx, ctx->tc_host, 4, 4)) return rc;
         for (int i = 0; i < 2; i++) CU(cudaEventCreateWithFlags(&ctx->tc_evt[i], cudaEventDisableTiming));
     }
     if (dev_block) *dev_block = ctx->tc;
@@ -3408,11 +3341,7 @@ static int mirror_create(b200sph_ctx *ctx)
                 CU(cudaMemcpyAsync(&tot, ctx->flag_b + n_sel, 4, cudaMemcpyDeviceToHost, ctx->stream));
                 CU(cudaStreamSynchronize(ctx->stream));
                 if (tot == 0) continue;
-                if ((int64_t)tot > sg.cap) {
-                    if (sg.idx) CU(cudaFree(sg.idx));
-                    sg.cap = (int64_t)tot + tot / 4 + 256;
-                    CU(cudaMalloc((void **)&sg.idx, 4 * (size_t)sg.cap));
-                }
+                if ((rc = grow(ctx, sg.idx, tot, (size_t)tot + tot / 4 + 256))) return rc;
                 k_save_idx<<<nb, 256, 0, ctx->stream>>>(n_sel, ctx->flag_a, ctx->flag_b, sg.idx);
                 LAUNCH_CHECK();
                 if ((rc = ensure_capacity(ctx, a, ai.n + tot))) return rc;   // may move the pool
@@ -3461,11 +3390,7 @@ int b200sph_halo_pack(b200sph_ctx *ctx, int arr, int slot, double lo, double hi,
     *count = tot;
     if ((int64_t)tot > cap) return set_err(ctx, "halo_pack: %u particles selected but the buffer holds %lld", tot, (long long)cap);
     if (slot == 0 || slot == 1) {  // remember the selection for halo_pack_selected
-        if ((int64_t)tot > ctx->halo_cap[arr][slot]) {
-            if (ctx->halo_idx[arr][slot]) CU(cudaFree(ctx->halo_idx[arr][slot]));
-            ctx->halo_cap[arr][slot] = (int64_t)tot + tot / 4 + 256;
-            CU(cudaMalloc((void **)&ctx->halo_idx[arr][slot], 4 * (size_t)ctx->halo_cap[arr][slot]));
-        }
+        if ((rc = grow(ctx, ctx->halo_idx[arr][slot], tot, (size_t)tot + tot / 4 + 256))) return rc;
         ctx->halo_cnt[arr][slot] = tot;
         if (tot) {
             k_save_idx<<<nb, 256, 0, ctx->stream>>>(n, ctx->flag_a, ctx->flag_b, ctx->halo_idx[arr][slot]);
@@ -3688,13 +3613,12 @@ int b200sph_peer_init(b200sph_ctx *ctx, int rank, int world, void *handle64)
     if (ctx->peer_box) return set_err(ctx, "peer_init: already initialised");
     int rc = peer_streams(ctx);
     if (rc) return rc;
-    const size_t box_bytes = std::max<size_t>(sizeof(PeerBox), 4096);
-    CU(cudaMalloc((void **)&ctx->peer_box, box_bytes));
-    CU(cudaMemset(ctx->peer_box, 0, box_bytes));
-    CU(cudaMalloc((void **)&ctx->peer_done, 2 * sizeof(unsigned)));
+    const size_t boxes = cdiv(4096, sizeof(PeerBox));   // at least a page
+    if ((rc = grow(ctx, ctx->peer_box, boxes, boxes)) || (rc = grow(ctx, ctx->peer_done, 2, 2)) ||
+        (rc = grow(ctx, ctx->peer_dec_dev, 1, 1)) || (rc = grow(ctx, ctx->peer_dec_host, 1, 1)))
+        return rc;
+    CU(cudaMemset(ctx->peer_box, 0, boxes * sizeof(PeerBox)));
     CU(cudaMemset(ctx->peer_done, 0, 2 * sizeof(unsigned)));
-    CU(cudaMalloc((void **)&ctx->peer_dec_dev, sizeof(double)));
-    CU(cudaHostAlloc((void **)&ctx->peer_dec_host, sizeof(PeerDecision), cudaHostAllocMapped));
     memset(ctx->peer_dec_host, 0, sizeof(PeerDecision));
     CU(cudaHostGetDevicePointer((void **)&ctx->peer_dec_hostdev, ctx->peer_dec_host, 0));
     cudaIpcMemHandle_t h;
@@ -3782,7 +3706,7 @@ int b200sph_peer_send(b200sph_ctx *ctx, int slot, int nb_rank, int side, double 
         // slot -1: the flag alone (this rank has no reusable build: the neighbour must not wait)
         A.prefix[a + 1] = A.prefix[a] + (slot < 0 ? 0 : ctx->halo_cnt[a][slot]);
         A.off[a] = ctx->arr[a].off;
-        A.idx[a] = slot < 0 ? nullptr : ctx->halo_idx[a][slot];
+        A.idx[a] = slot < 0 ? nullptr : ctx->halo_idx[a][slot].p;
     }
     const int64_t tot = A.prefix[ctx->narr];
     if (tot * halo_nf(ctx) > cap_doubles) return set_err(ctx, "peer_send: staging buffer too small");
@@ -3883,10 +3807,10 @@ int b200sph_peer_recv(b200sph_ctx *ctx, int side, const int64_t *ghost_first, co
     const bool records = repack && ctx->state_packed && !elastic_allocated(ctx);
     GhostPackArgs R;
     memset(&R, 0, sizeof(R));
-    R.rank = repack ? ctx->rank : nullptr;
+    R.rank = repack ? ctx->rank.p : nullptr;
     R.skey = ctx->skey;
     R.A = ctx->A; R.AB = ctx->AB;
-    R.C = records ? ctx->C : nullptr;
+    R.C = records ? ctx->C.p : nullptr;
     R.G = ctx->G;
     R.ptype = ctx->ptype;
     R.p = f32_ptr(ctx, B200SPH_P); R.cs = f32_ptr(ctx, B200SPH_CS);
@@ -4069,7 +3993,7 @@ int b200sph_migrate_out(b200sph_ctx *ctx, int arr, double lo, double hi, double 
         const int p = f < mnf ? migrate_msg[f] : (f == mnf ? B200SPH_TAG : B200SPH_PID);
         const size_t esz = prop_kind(p).size();
         if (esz == 8) k_gather_f64<<<nb, 256, 0, ctx->stream>>>(f64_ptr(ctx, p), off, n, ctx->flag_a, ctx->flag_b, ctx->stage_buf, 0);
-        else k_gather_u32<<<nb, 256, 0, ctx->stream>>>(u32_ptr(ctx, p), off, n, ctx->flag_a, ctx->flag_b, (uint32_t *)ctx->stage_buf);
+        else k_gather_u32<<<nb, 256, 0, ctx->stream>>>(u32_ptr(ctx, p), off, n, ctx->flag_a, ctx->flag_b, (uint32_t *)ctx->stage_buf.p);
         LAUNCH_CHECK();
         if (keep) CU(cudaMemcpyAsync((char *)ctx->prop[p] + esz * (size_t)off, ctx->stage_buf, esz * (size_t)keep, cudaMemcpyDeviceToDevice, ctx->stream));
     }

@@ -102,6 +102,14 @@ int ipc_import(void **p, const void *handle64)
 
 int ipc_release(void *p) { return dev_free(p); }
 
+// the number of live "device" and pinned blocks (imported IPC mappings included): what a
+// destroyed context must give back
+extern "C" long long emu_live_blocks()
+{
+    std::lock_guard<std::mutex> g(g_blocks_mu);
+    return (long long)g_blocks.size();
+}
+
 thread_local idx3 t_threadIdx, t_blockIdx, t_blockDim, t_gridDim;
 thread_local WarpCtx *t_warp = nullptr;
 thread_local BlockCtx *t_block = nullptr;
