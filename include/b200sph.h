@@ -402,7 +402,7 @@ int b200sph_stage_edac(b200sph_ctx *ctx, int arr, int which, double dt);
 int b200sph_stage_edac_dev(b200sph_ctx *ctx, int arr, int which);
 
 /* The elastic-dynamics evaluation (see b200sph_solid_program); same neighbour lists as
- * pair_pass.  NOT YET RUN ON HARDWARE (see the property block above). */
+ * pair_pass. */
 int b200sph_solid_pass(b200sph_ctx *ctx, const b200sph_solid_program *prog,
                        int64_t *pairs_out);
 /* SolidMechStep integrator_step.py:173-252 (e / ae are not mirrored: the scheme has no

@@ -322,7 +322,7 @@ class Oracle(object):
     def stage_edac(self, arr, which, dt):
         self.lib.orc_stage_edac(self.h, arr, which, dt)
 
-    # -- elastic dynamics (oracle only so far) ----------------------------------
+    # -- elastic dynamics -------------------------------------------------------
     def solid_program(self, elastic, sources, eps=0.3, alpha=1.0, beta=1.0,
                       eps_xsph=0.5, grad3d=False):
         P = OrcSolidProgram()

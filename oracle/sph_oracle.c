@@ -1156,7 +1156,7 @@ void orc_stage_edac(orc_ctx *c, int arr, int which, double dt)
 }
 
 /* ------------------------------------------------------------------------ */
-/* elastic dynamics (SURVEY.md 8f-2): oracle only                             */
+/* elastic dynamics (SURVEY.md 8f-2)                                         */
 /* ------------------------------------------------------------------------ */
 
 /* cyclic Jacobi; converges to machine precision in < 10 sweeps for 3x3 */

@@ -185,7 +185,8 @@ void orc_stage_tvf(orc_ctx *, int arr, int which, double dt);
 /* EDACStep wc/edac.py:82-133 (the external-flow branch: x moves with the XSPH velocity ax) */
 void orc_stage_edac(orc_ctx *, int arr, int which, double dt);
 
-/* elastic dynamics (Gray et al.), SURVEY.md 8f-2 -- ORACLE ONLY so far, no CUDA yet.
+/* elastic dynamics (Gray et al.), SURVEY.md 8f-2; the reference of k_solid_pass1/2 and
+ * k_stage_solid (tests/test_gpu_solid_oracle.py).
  * group 1: IsothermalEOS (solid_mech/basic.py:93-101), VelocityGradient2D/3D
  * (basic_equations.py:67-148), MonaghanArtificialStress (:104-242);
  * group 2: ContinuityEquation, MomentumEquationWithStress (:245-387),

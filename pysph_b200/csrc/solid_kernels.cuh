@@ -3,8 +3,8 @@
 // stand-alone header).
 
 // --------------------------------------------------------------------------
-// Elastic dynamics (solid_mech/basic.py:604-651), elastic arrays only.  NOT YET RUN ON
-// HARDWARE.  Sorted records: AB = {A, B}, C3 = (rho, p, cs, type) [ctx->C], and the
+// Elastic dynamics (solid_mech/basic.py:604-651), elastic arrays only.  Sorted records:
+// AB = {A, B}, C3 = (rho, p, cs, type) [ctx->C], and the
 // stress records T = (s - p I) / rho^2 and R (artificial stress), 6 components each:
 //   T01 = (T00, T01, T02, T11)   T2R = (T12, T22, R00, R01)   R2 = (R02, R11, R12, R22)
 // --------------------------------------------------------------------------

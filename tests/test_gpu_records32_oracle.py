@@ -64,11 +64,11 @@ def _eos_calls(variant):
     return [(0, RHO0, C0, 7.0, P0)] * len(NAMES)
 
 
-def _positions(dim, radius, rs, dx):
-    """A jittered lattice with a cluster at twice the density in one corner, a sparse region
-    in the opposite corner, two particles at the same position and one (the first) far from
-    all others.  Returns (positions, indices of the coincident pair)."""
-    nside = {1: 60, 2: 16, 3: 8}[dim]
+def _positions(dim, radius, rs, dx, nside=None):
+    """A jittered lattice (nside particles a side) with a cluster at twice the density in one
+    corner, a sparse region in the opposite corner, two particles at the same position and
+    one (the first) far from all others.  Returns (positions, indices of the coincident pair)."""
+    nside = nside or {1: 60, 2: 16, 3: 8}[dim]
     g = np.mgrid[tuple(slice(0, nside) for _ in range(dim))].reshape(dim, -1).T * dx
     corner = np.all(g < 4 * dx, axis=1)
     sparse = np.all(g >= (nside - 4) * dx, axis=1) & (rs.uniform(size=len(g)) < 0.7)

@@ -392,7 +392,7 @@ def test_edac_tvf_step_matches_reference_bodies():
 
 
 # ---------------------------------------------------------------------------
-# elastic dynamics (SURVEY.md 8f-2): ORACLE ONLY so far -- the restatement of
+# elastic dynamics (SURVEY.md 8f-2): the restatement of
 # ElasticSolidsScheme's loops against the reference's scheme method + bodies, with the
 # reference's own compiled linalg3 eigen solver behind MonaghanArtificialStress
 # ---------------------------------------------------------------------------
