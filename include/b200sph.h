@@ -354,6 +354,34 @@ enum {
 int b200sph_density_filter(b200sph_ctx *ctx, uint32_t array_mask, int mode, int kernel, int rhotmp_prop,
                            int real_only);
 
+/* ---- particle shifting: ShiftPositions (pysph/sph/wc/shift.py:191-271) ----------------------
+ * b200sph_shift: the Group([SimpleShift(a, [a])]) or Group([FickianShift(a, [a])]) of every array
+ *   a of array_mask, on its real particles, with the evaluation's kernel (b200sph_set_kernel).
+ *   Sources are the array's own particles, the particle itself and its periodic images
+ *   included.  Every dpos is formed from the positions before the shift, then x += dpos (a
+ *   Jacobi update).  SIMPLE: dpos = coef ri^2 vmax dt sum x_ij / (r_ij^3 + 1e-8), vmax = max |v|
+ *   over the array, reduced on the device.  FICKIAN: dpos = -coef h_i |v_i| dt
+ *   sum (m_j / rho_j) (1 + f_ij) grad W_ij, f_ij = tensile_R (W_ij / W(h_i / hdx, h_i))^tensile_n
+ *   when `tensile`, else 0.  x_ij, r^2 and the accept test are fp64.  dpos stays on the device.
+ * b200sph_correct_velocities: CorrectVelocities on the arrays of array_mask, each shifted by the
+ *   last b200sph_shift and the neighbour search updated since: u_i[k] += sum_l gradv[3 k + l]
+ *   dpos_i[l], gradv[3 b + a] = -sum (m_j / rho_j) v_ij[a] DW_ij[b] (the reference's body as
+ *   written: the transpose of grad v is applied to dpos).
+ * pairs: if not null, receives the accepted entries (the destinations' N_NBRS summed; the call
+ *   then waits for it), like b200sph_pair_pass.
+ * Afterwards the packed records are stale (and, after a shift, the neighbour search: the next
+ * nnps_update judges the moved positions by its drift check).  Refused: an unknown kind, a bad
+ * mask, mirror domains, the slab decomposition, a stale neighbour search, lists that cannot
+ * index the particles, and a correction of an array without a shift since its particle set last
+ * changed.  New symbols only: B200SPH_ABI_VERSION stays 6. */
+enum {
+    B200SPH_SHIFT_SIMPLE = 0,
+    B200SPH_SHIFT_FICKIAN = 1
+};
+int b200sph_shift(b200sph_ctx *ctx, uint32_t array_mask, int kind, double dt, double coef, double hdx,
+                  int tensile, double tensile_R, double tensile_n, int64_t *pairs);
+int b200sph_correct_velocities(b200sph_ctx *ctx, uint32_t array_mask, int64_t *pairs);
+
 /* ---- interpolation at probe points: Interpolator (pysph/tools/interpolator.py:18-510) -------
  * b200sph_probe_create: n points (x, y, z, host fp64, copied) with the probes' smoothing length h
  *   (the Interpolator's: the largest h of its arrays when the points were set).  Returns the id

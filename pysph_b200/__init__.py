@@ -15,7 +15,7 @@ DeviceHelper (``pa.gpu``)   :class:`B200DeviceHelper` / :class:`B200Backend`
 Equation / Group            :mod:`pysph_b200.equations`
 WCSPHScheme.get_equations   :class:`pysph_b200.scheme.WCSPHScheme`
 Solver step loop            :class:`B200Solver`
-solver tools                :class:`DensityCorrection`
+solver tools                :class:`DensityCorrection`, :class:`ShiftPositions`
 tools.interpolator          :class:`Interpolator`
 ParallelManager             :class:`pysph_b200.parallel.SlabParallelManager`
 ==========================  ==================================================
@@ -42,6 +42,7 @@ from .integrator import (B200Integrator, PECIntegrator, EPECIntegrator,
                          TVDRK3Integrator, WCSPHStep, WCSPHTVDRK3Step)
 from .solver import B200Solver
 from .tools import Tool, DensityCorrection
+from .shift import SimpleShift, FickianShift, CorrectVelocities, ShiftPositions
 from .interpolator import Interpolator, get_bounding_box, get_nx_ny_nz
 from .edac import EDACScheme, EDACTVFStep, EDACStep
 from .output import dump, load

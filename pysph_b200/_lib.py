@@ -3,6 +3,7 @@
 Loading fails loudly if the shared library is missing -- there is no CPU or
 PyTorch fallback for any entry point.
 """
+import gc
 import ctypes as C
 import os
 
@@ -52,6 +53,9 @@ EQ_LAMINAR = 32
 
 # density re-initialisation filters (B200SPH_DFILTER_*)
 DFILTER_SHEPARD, DFILTER_MLS2D, DFILTER_MLS3D = 0, 1, 2
+
+# particle shifting (B200SPH_SHIFT_*)
+SHIFT_SIMPLE, SHIFT_FICKIAN = 0, 1
 
 # interpolation methods (B200SPH_INTERP_*), by the Interpolator's method names
 INTERP_METHODS = {'shepard': 0, 'sph': 1, 'splash': 2, 'splash_norm': 3, 'order1': 4}
@@ -161,6 +165,9 @@ SIGNATURES = {
     'b200sph_generic_launch': (C.c_int, [_ctx_p, C.c_int, C.c_char_p, C.c_int, C.c_int, C.c_uint,
                                          C.c_int, C.c_double, C.c_double, C.c_int]),
     'b200sph_density_filter': (C.c_int, [_ctx_p, C.c_uint32, C.c_int, C.c_int, C.c_int, C.c_int]),
+    'b200sph_shift': (C.c_int, [_ctx_p, C.c_uint32, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int,
+                                C.c_double, C.c_double, C.POINTER(_i64)]),
+    'b200sph_correct_velocities': (C.c_int, [_ctx_p, C.c_uint32, C.POINTER(_i64)]),
     'b200sph_probe_create': (C.c_int, [_ctx_p, _i64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double]),
     'b200sph_probe_release': (C.c_int, [_ctx_p, C.c_int]),
     'b200sph_interpolate': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int),
@@ -241,6 +248,10 @@ def load():
             'pysph_b200: %s is missing. Build it with `python -m '
             'pysph_b200.build` (needs nvcc). There is no CPU fallback.'
             % LIB_PATH)
+    # contexts that only reference cycles still hold (a solver and the tools registered on it)
+    # keep their device memory until the cyclic collector runs: release them before a library
+    # is taken into use, not at an arbitrary later allocation
+    gc.collect()
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)   # AttributeError if the symbol is missing

@@ -144,6 +144,14 @@ class B200AccelerationEval(object):
             elif kind == 'dfilter':
                 _, mode, mask, real_only = op
                 ctx.call('b200sph_density_filter', mask, mode, self._kid, self._rhotmp, real_only)
+            elif kind == 'shift':
+                _, skind, mask, coef, hdx, tensile, tR, tn = op
+                ctx.call('b200sph_shift', mask, skind, float(dt), coef, hdx, tensile, tR, tn,
+                         C.byref(cnt) if self.count_pairs else None)
+                self._pairs += cnt.value if self.count_pairs else 0
+            elif kind == 'correct_vel':
+                ctx.call('b200sph_correct_velocities', op[1], C.byref(cnt) if self.count_pairs else None)
+                self._pairs += cnt.value if self.count_pairs else 0
             elif kind == 'update_nnps':
                 # mako:139-145: nnps.update_domain(); nnps.update()
                 ctx.call('b200sph_update_domain')

@@ -22,7 +22,7 @@
 // One translation unit: this file holds the context, the pool and every C-ABI entry
 // point; the kernels are included below by family (pool_kernels, scan, nnps_kernels,
 // sph_kernels, pair_kernel, pair_list, tvf_kernels, solid_kernels, halo_kernels, density_filter,
-// interp_kernels .cuh).
+// interp_kernels, shift_kernels .cuh).
 //
 // No CPU fallback: every entry point needs a CUDA device.
 #include "b200sph.h"
@@ -245,6 +245,7 @@ template <class T, Mem M = Mem::DEVICE> struct Buf {
 };
 struct PeerBox;
 struct PeerDecision;
+struct ShiftRec;    // shift_kernels.cuh
 
 struct b200sph_ctx {
     int device = 0;
@@ -416,6 +417,13 @@ struct b200sph_ctx {
     Buf<float> interp_rho;
     Buf<unsigned> interp_red;
     Buf<double> interp_out;
+    // particle shifting (b200sph_shift, b200sph_correct_velocities): the fp64 records [n_sorted]
+    // each, dpos and the velocity change [3 pool_end] by gid, max |v| per array; shift_mask: the
+    // arrays whose dpos is in shift_dpos
+    Buf<ShiftRec> shift_P, shift_V;
+    Buf<double> shift_dpos, shift_dvel;
+    Buf<long long> shift_vmax;
+    unsigned shift_mask = 0;
     // Group(start_idx, stop_idx): one-shot destination ranges of the next pair pass
     int64_t dst_lo[B200SPH_MAX_ARRAYS] = {0}, dst_hi[B200SPH_MAX_ARRAYS] = {0};
     bool dst_ranged = false;
@@ -512,6 +520,7 @@ static void set_changed(b200sph_ctx *ctx)
     state_changed(ctx);
     ctx->ptype_dirty = true, ctx->h_dirty = true;
     ctx->hm_known = false;
+    ctx->shift_mask = 0;   // the gids of the last shift's dpos may name other particles now
 }
 
 // Particles arrived or left with their own h (halo_append, migrate_out, mirror images): the
@@ -683,6 +692,7 @@ __device__ __forceinline__ void rec32_make(const float4 A, const double u, const
 #include "halo_kernels.cuh"
 #include "density_filter.cuh"
 #include "interp_kernels.cuh"
+#include "shift_kernels.cuh"
 
 // --------------------------------------------------------------------------
 // host side
@@ -2348,6 +2358,136 @@ int b200sph_density_filter(b200sph_ctx *ctx, uint32_t array_mask, int mode, int 
         ctx->stats.kernel_launches += 2;
     }
     // rho changed: the next evaluation packs its records (and applies its EOS) from it
+    state_changed(ctx);
+    ctx->spec_records = false;
+    return 0;
+}
+
+// ---- particle shifting (shift_kernels.cuh) ---------------------------------------------------
+// The checks, the invalidation rules and the records both entry points share.  Like
+// density_filter, a list consumer that writes pool properties between evaluations: the deferred
+// initialize has copied what it overwrites (ensure_pool: the write lands in the live x after the
+// x / x0 rename), the pending EOS calls are in the pool, the lists cover the array's own pairs.
+// The records are packed from the current pool.
+static int shift_prepare(b200sph_ctx *ctx, const char *who, uint32_t array_mask, ShiftArgs &sa)
+{
+    if (int rcc = require_confirmed(ctx, who)) return rcc;
+    CU(cudaSetDevice(ctx->device));
+    int rc = ensure_pool(ctx);
+    if (rc) return rc;
+    if (array_mask == 0 || array_mask >= (1u << ctx->narr)) return set_err(ctx, "%s: bad array mask 0x%x", who, array_mask);
+    if (ctx->peer_box || ctx->comm_pending) return set_err(ctx, "%s runs on one GPU (no slab decomposition)", who);
+    if (mirror_any(ctx)) return set_err(ctx, "%s: mirror domains are not supported", who);
+    if (!ctx->grid_valid) return set_err(ctx, "%s: the NNPS is stale (particles were pushed, resized or moved); call nnps_update first", who);
+    if ((rc = eos_flush(ctx)) || (rc = ab_positions(ctx))) return rc;
+    memset(&sa, 0, sizeof(sa));
+    if (ctx->n_sorted == 0) return 0;
+    unsigned long long want[B200SPH_MAX_ARRAYS] = {0};
+    for (int a = 0; a < ctx->narr; a++)
+        if ((array_mask >> a) & 1u) want[a] |= 0xFFull << (8 * a);
+    char refusal[96];
+    snprintf(refusal, sizeof(refusal), "%s: the neighbour lists cannot index the particles", who);
+    if ((rc = prepare_lists(ctx, want, refusal))) return rc;
+    const size_t n = (size_t)ctx->n_sorted, np = 3 * (size_t)ctx->pool_end;
+    if ((rc = grow(ctx, ctx->shift_P, n, n)) || (rc = grow(ctx, ctx->shift_V, n, n)) ||
+        (rc = grow(ctx, ctx->shift_dpos, np, np)) || (rc = grow(ctx, ctx->shift_dvel, np, np)) ||
+        (rc = grow(ctx, ctx->shift_vmax, B200SPH_MAX_ARRAYS, B200SPH_MAX_ARRAYS)))
+        return rc;
+    sa.P = ctx->shift_P; sa.V = ctx->shift_V;
+    sa.perm = ctx->perm; sa.cnt = ctx->cnt; sa.lst = ctx->lst; sa.skey = ctx->skey; sa.stype = ctx->stype;
+    sa.x = f64_ptr(ctx, B200SPH_X); sa.y = f64_ptr(ctx, B200SPH_Y); sa.z = f64_ptr(ctx, B200SPH_Z);
+    sa.u = f64_ptr(ctx, B200SPH_U); sa.v = f64_ptr(ctx, B200SPH_V); sa.w = f64_ptr(ctx, B200SPH_W);
+    sa.h = f64_ptr(ctx, B200SPH_H); sa.m = f64_ptr(ctx, B200SPH_M); sa.rho = f64_ptr(ctx, B200SPH_RHO);
+    sa.dpos = ctx->shift_dpos; sa.dvel = ctx->shift_dvel; sa.vmax = ctx->shift_vmax;
+    sa.n = ctx->n_sorted; sa.capg = ctx->capg;
+    sa.ncx = ctx->G.nc[0]; sa.ncy = ctx->G.nc[1]; sa.zorder = ctx->G.zorder;
+    for (int d = 0; d < 3; d++) {
+        sa.per[d] = ctx->G.periodic[d];
+        sa.L[d] = ctx->dom_hi[d] - ctx->dom_lo[d];
+    }
+    sa.kr = ctx->radius_scale;
+    sa.kfac = kernel_fac(ctx->kernel, ctx->dim);
+    sa.mask = array_mask;
+    k_shift_pack<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(sa);
+    LAUNCH_CHECK();
+    return 0;
+}
+
+// ShiftPositions' shift Group: dpos of every real particle of the arrays in array_mask from the
+// positions before the shift, then x += dpos.  The moved positions are judged by the next
+// nnps_update's drift check against the build, like any other motion.
+int b200sph_shift(b200sph_ctx *ctx, uint32_t array_mask, int kind, double dt, double coef, double hdx, int tensile,
+                  double tensile_R, double tensile_n, int64_t *pairs)
+{
+    if (kind != B200SPH_SHIFT_SIMPLE && kind != B200SPH_SHIFT_FICKIAN) return set_err(ctx, "shift: unknown kind %d", kind);
+    if (kind == B200SPH_SHIFT_FICKIAN && tensile && !(hdx > 0.0)) return set_err(ctx, "shift: FickianShift needs hdx > 0 (got %g)", hdx);
+    ShiftArgs sa;
+    int rc = shift_prepare(ctx, "shift", array_mask, sa);
+    if (rc) return rc;
+    if (ctx->n_sorted > 0) {
+        PhaseTimer pt(ctx, 1);
+        if ((rc = pairs_arm(ctx, pairs, &sa.pair_counter))) return rc;
+        sa.dt = dt; sa.coef = coef; sa.hdx = hdx; sa.tensile = tensile; sa.tR = tensile_R; sa.tn = tensile_n;
+        if (kind == B200SPH_SHIFT_SIMPLE) {
+            // SimpleShift.py_initialize: vmax of each array, on the device
+            CU(cudaMemsetAsync(ctx->shift_vmax, 0, sizeof(long long) * B200SPH_MAX_ARRAYS, ctx->stream));
+            for (int a = 0; a < ctx->narr; a++)
+                if (((array_mask >> a) & 1u) && ctx->arr[a].n > 0) {
+                    k_shift_vmax<<<(unsigned)cdiv(ctx->arr[a].n, 256), 256, 0, ctx->stream>>>(
+                        sa.u, sa.v, sa.w, ctx->arr[a].off, ctx->arr[a].n, ctx->shift_vmax + a);
+                    LAUNCH_CHECK();
+                }
+        }
+        const unsigned nb = (unsigned)cdiv(ctx->n_sorted, SHIFT_NT);
+        rc = with_kernel_dim(ctx, "shift", [&](auto kc, auto dc) {
+            constexpr int K = decltype(kc)::value, D = decltype(dc)::value;
+            if (kind == B200SPH_SHIFT_SIMPLE) k_shift<K, D, B200SPH_SHIFT_SIMPLE><<<nb, SHIFT_NT, 0, ctx->stream>>>(sa);
+            else k_shift<K, D, B200SPH_SHIFT_FICKIAN><<<nb, SHIFT_NT, 0, ctx->stream>>>(sa);
+            LAUNCH_CHECK();
+            return 0;
+        });
+        if (rc) return rc;
+        k_shift_apply<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(sa, sa.dpos, sa.x, sa.y, sa.z);
+        LAUNCH_CHECK();
+        if ((rc = pairs_read(ctx, pairs))) return rc;
+    } else if (pairs) {
+        *pairs = 0;
+    }
+    ctx->shift_mask = array_mask;
+    // x changed: the grid, the packed positions and the records made from them are stale
+    particles_moved(ctx);
+    ctx->spec_records = false;
+    return 0;
+}
+
+// ShiftPositions' CorrectVelocities Group, after the neighbour search has seen the shifted
+// positions: u += gradv . dpos with the dpos of the last b200sph_shift of these arrays.
+int b200sph_correct_velocities(b200sph_ctx *ctx, uint32_t array_mask, int64_t *pairs)
+{
+    if (array_mask & ~ctx->shift_mask)
+        return set_err(ctx, "correct_velocities: no shift of the arrays 0x%x since the particle set last changed (call b200sph_shift first)",
+                       array_mask & ~ctx->shift_mask);
+    ShiftArgs sa;
+    int rc = shift_prepare(ctx, "correct_velocities", array_mask, sa);
+    if (rc) return rc;
+    if (ctx->n_sorted > 0) {
+        PhaseTimer pt(ctx, 1);
+        if ((rc = pairs_arm(ctx, pairs, &sa.pair_counter))) return rc;
+        const unsigned nb = (unsigned)cdiv(ctx->n_sorted, SHIFT_NT);
+        rc = with_kernel_dim(ctx, "correct_velocities", [&](auto kc, auto dc) {
+            constexpr int K = decltype(kc)::value, D = decltype(dc)::value;
+            k_correct_velocities<K, D><<<nb, SHIFT_NT, 0, ctx->stream>>>(sa);
+            LAUNCH_CHECK();
+            return 0;
+        });
+        if (rc) return rc;
+        k_shift_apply<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(sa, sa.dvel, sa.u, sa.v, sa.w);
+        LAUNCH_CHECK();
+        if ((rc = pairs_read(ctx, pairs))) return rc;
+    } else if (pairs) {
+        *pairs = 0;
+    }
+    // u, v, w changed: the next evaluation packs its records from them
     state_changed(ctx);
     ctx->spec_records = false;
     return 0;

@@ -10,6 +10,8 @@ recognises each equation by *class name* and maps every Group onto
     ('pair', PairProgram)                                  fused pair kernel
     ('update_nnps',)                                       Group(update_nnps=True)
     ('dfilter', mode, array_mask, real_only)              density re-initialisation
+    ('shift', kind, array_mask, coef, hdx, tensile, R, n)  particle shifting (dt: compute's)
+    ('correct_vel', array_mask)                            CorrectVelocities after a shift
 
 Anything the CUDA library has no kernel for raises NotImplementedError here,
 i.e. at setup time, never silently at run time.
@@ -65,9 +67,13 @@ DFILTER_EQUATIONS = {
 
 # every equation that has a hand-written kernel; a Group made ONLY of others takes the
 # generic-equation fallback (pysph_b200/codegen.py)
+# particle shifting (wc/shift.py): a Group of one of them -> ('shift', ...) / ('correct_vel', ...)
+# ops (k_shift, k_correct_velocities)
+SHIFT_EQUATIONS = ('SimpleShift', 'FickianShift', 'CorrectVelocities')
+
 KNOWN_EQUATIONS = set(PAIR_EQUATIONS) | set(NO_SOURCE_EQUATIONS) | set(TVF_GROUP1) | \
     set(TVF_WALL) | set(TVF_WALL_OPTIONAL) | set(TVF_GROUP2) | set(SOLID_GROUP1) | \
-    set(SOLID_GROUP2) | set(DFILTER_EQUATIONS)
+    set(SOLID_GROUP2) | set(DFILTER_EQUATIONS) | set(SHIFT_EQUATIONS)
 import itertools
 _generic_uid = itertools.count()
 
@@ -533,12 +539,45 @@ def _build_dfilter(g, index, ranged):
     return [('dfilter', DFILTER_EQUATIONS[names[0]], mask, real_only)]
 
 
+def _build_shift(g, index, ranged):
+    """A Group of SimpleShift / FickianShift or of CorrectVelocities, each with its destination
+    as its only source (what ShiftPositions builds, shift.py:227-262) -> one ('shift', ...) or
+    ('correct_vel', ...) op per equation.  The shifts' dt is the one compute(t, dt) is given, as
+    SPHEvaluator.evaluate(dt=...) passes it."""
+    names = sorted(set(_eq_name(e) for e in g.equations))
+    if len(names) != 1 or names[0] not in SHIFT_EQUATIONS:
+        raise NotImplementedError(
+            'B200 backend: a shift equation (%s) cannot share a Group with other equations or '
+            'another shift equation; got %s' % (', '.join(SHIFT_EQUATIONS), names))
+    _no_range(g, ranged, 'particle-shifting')
+    ops = []
+    for eq in g.equations:
+        if eq.dest not in index:
+            raise ValueError('equation %s: unknown destination array %r' % (names[0], eq.dest))
+        if list(eq.sources or []) != [eq.dest]:
+            raise NotImplementedError(
+                'B200 backend: %s(dest=%r, sources=%r): the shift takes its destination as its '
+                'only source' % (names[0], eq.dest, eq.sources))
+        mask = 1 << index[eq.dest]
+        if names[0] == 'SimpleShift':
+            ops.append(('shift', _lib.SHIFT_SIMPLE, mask, float(eq.beta), 1.0, 0, 0.0, 0.0))
+        elif names[0] == 'FickianShift':
+            ops.append(('shift', _lib.SHIFT_FICKIAN, mask, float(eq.fickian_const), float(eq.hdx),
+                        1 if eq.tensile_correction else 0, float(eq.tensile_const),
+                        float(eq.tensile_pow)))
+        else:
+            ops.append(('correct_vel', mask))
+    return ops
+
+
 def _leaf_body(g, index, arrays, particle_arrays):
     ops = []
     start, stop = getattr(g, 'start_idx', 0), getattr(g, 'stop_idx', None)
     ranged = (stop is not None) or (start not in (0, None))
     if any(_eq_name(e) in DFILTER_EQUATIONS for e in g.equations):
         return _build_dfilter(g, index, ranged)
+    if any(_eq_name(e) in SHIFT_EQUATIONS for e in g.equations):
+        return _build_shift(g, index, ranged)
     from . import codegen
     # a Group with at least one equation the library has no kernel for, all of whose equations
     # carry Python bodies (the reference's own objects always do; this package's descriptors of
