@@ -243,7 +243,9 @@ int b200sph_set_async_copies(b200sph_ctx *ctx, int on);
 /* device pointer of a property region of one array (for zero-copy use by
  * torch / NCCL plumbing); fp64 props -> double*, fp32 props -> float*.
  * The pointers of x .. rho and x0 .. rho0 hold until the next stage call: a stage 1 may
- * exchange the buffers behind the two sets of names instead of copying one into the other. */
+ * exchange the buffers behind the two sets of names instead of copying one into the other.
+ * Those of au .. az hold until the next pair pass: the pass after such a stage 1 may write
+ * into a second set of buffers, which then goes by these names. */
 int b200sph_device_ptr(b200sph_ctx *ctx, int arr, int prop, void **out);
 
 /* ---- NNPS: kernel choice, DomainManager.update, NNPS.update ------------- */
@@ -469,8 +471,11 @@ int b200sph_time_get(b200sph_ctx *ctx, double out[2]);
  * rho / p / cs change only when the next evaluation issues its b200sph_eos calls.  On the same
  * path which = 0 (initialize) launches nothing: the next fused stage copies x .. rho into
  * x0 .. rho0 as it goes, and applies the pool side of the last evaluation's EOS calls (the
- * pair pass leaves it to that kernel).  Every other entry point that could observe either runs
- * it first, so what the host can pull is the same as with the separate kernels. */
+ * pair pass leaves it to that kernel).  A stage 1 that exchanges the buffers (no ghosts) does
+ * not even store x .. rho, nor p / cs of those EOS calls: stage 2 reads none of them but rho,
+ * which it forms again as stage 1 did.  Every other
+ * entry point that could observe any of this forms it first, from the operands the stage
+ * read, so what the host can pull is the same as with the separate kernels. */
 int b200sph_stage_dev(b200sph_ctx *ctx, int arr, int which);
 /* WCSPHTVDRK3Step integrator_step.py:96-168 (TVDRK3Integrator, integrator.py:426-460); which:
  * 0 initialize (WCSPHStep's), 1 stage1 q = q0 + dt aq, 2 stage2 q = 3/4 q0 + 1/4 (q + dt aq),
@@ -664,6 +669,9 @@ int b200sph_reset_stats(b200sph_ctx *ctx);
  * (k_pair_list_r32: the WCSPH Group, uniform h and m, one Tait EOS with gamma = 7, no
  * ghosts; B200SPH_RECORDS=48 turns them off) */
 int b200sph_records32_launches(b200sph_ctx *ctx, int64_t *out);
+/* how many half steps (since the last reset) a fused WCSPHStep stage 1 left pending had to be
+ * formed after all, because something read or changed x .. rho, p or cs before stage 2 */
+int b200sph_half_materialised(b200sph_ctx *ctx, int64_t *out);
 /* per-phase CUDA-event timing: 0 off, 1 every phase (ms_nnps, ms_pair, ms_other),
  * 2 the pair kernels only (ms_pair; two events per pair pass instead of ~25 per
  * step).  Event pairs are recorded on the stream (no sync) and resolved by

@@ -248,6 +248,8 @@ class B200Backend(object):
         n32 = C.c_int64()
         self.ctx.call('b200sph_records32_launches', C.byref(n32))
         out['pair_launches_r32'] = n32.value
+        self.ctx.call('b200sph_half_materialised', C.byref(n32))
+        out['half_materialised'] = n32.value
         return out
 
     def synchronize(self):

@@ -450,6 +450,21 @@ struct b200sph_ctx {
     bool dt_adaptive_seen = false;  // a dt proposal followed the last stage2: reduce in the next one
     bool init_pending = false;   // an initialize of every array waits for the next fused stage (init_materialise)
     int64_t n_fused = 0;
+    // a fused WCSPHStep stage 1 left x .. rho and the pool side of its EOS calls unwritten
+    // (half_materialise forms them from what the stage read: its factor, its EOS calls)
+    bool half_pending = false;
+    double half_f = 0.0;
+    const double *half_tc = nullptr;
+    int half_eos = 0;
+    EosTab half_EP;
+    int64_t n_half_materialised = 0;
+    // the second set of arho, au .. az (acc_swap); acc_swapped: the pair pass after that stage 1 writes
+    // into it, and acc_spare holds the accelerations the stage read.  acc_differ: where the two
+    // sets may hold different values (ACC_* bits); the pair passes do not write every array's
+    // accelerations, and the ones they leave must be the same in both sets
+    Buf<float> acc_spare[7];   // arho, au .. az: the property ids B200SPH_ARHO .. B200SPH_AZ
+    bool acc_swapped = false;
+    unsigned acc_differ = ~0u;
 
     // stats
     b200sph_stats stats;
@@ -800,6 +815,8 @@ static int pool_layout(b200sph_ctx *ctx, const int64_t *new_cap)
     if (elastic_allocated(ctx))
         for (Buf<float4> *b : {&ctx->T01, &ctx->T2R, &ctx->R2})
             if ((rc = grow(ctx, *b, n, n))) return rc;
+    for (Buf<float> &b : ctx->acc_spare) CU(b.reset());   // (acc_swap allocates it again, at pool_cap)
+    ctx->acc_differ = ~0u;
     return 0;
 }
 
@@ -841,17 +858,21 @@ static int sync_comm(b200sph_ctx *ctx)
     return 0;
 }
 
-static int init_materialise(b200sph_ctx *ctx);
+static int materialise_pending(b200sph_ctx *ctx);
 // every entry point starts here; all but those of the time step's fast path (pair_pass, eos,
-// nnps_update, the WCSPH stages: keep_init) first run a deferred initialize
+// nnps_update, the WCSPH stages, update_domain, the dt reductions: keep_init) first run a
+// deferred initialize or half step, and, as they may write accelerations, no longer count on
+// the spare acceleration set matching the slots
 static int ensure_pool(b200sph_ctx *ctx, bool join = true, bool keep_init = false)
 {
     if (join) {
         int rc0 = sync_comm(ctx);
         if (rc0) return rc0;
     }
-    if (!keep_init)
-        if (int rci = init_materialise(ctx)) return rci;
+    if (!keep_init) {
+        if (int rci = materialise_pending(ctx)) return rci;
+        ctx->acc_differ = ~0u;
+    }
     if (ctx->pool_cap == 0) {
         int64_t caps[B200SPH_MAX_ARRAYS];
         for (int a = 0; a < ctx->narr; a++) caps[a] = std::max(ctx->arr[a].cap, ctx->arr[a].n);
@@ -987,6 +1008,94 @@ static int init_materialise(b200sph_ctx *ctx)
         k_stage<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
         LAUNCH_CHECK();
     }
+    return 0;
+}
+
+// ---- the deferred half step ------------------------------------------------------------------
+// WCSPHStep.stage2 computes q = q0 + dt aq from x0 .. rho0 and the second evaluation's
+// accelerations, and that evaluation reads the predicted state from the 32-byte records: in a
+// step that nothing observes between the stages nobody reads the predicted x .. w, nor the p / cs
+// that stage 1 formed from rho0 (stage 2 writes them again); the predicted rho only feeds stage
+// 2's EOS calls, and stage 2 can form it again as stage 1 did.  So the fused stage 1 that takes
+// the initialize by renaming (init_by_rename) and writes the 32-byte records leaves them unwritten
+// (half_pending, 64 B per particle less to store) and the host keeps what forms them: the stage's
+// factor and its EOS calls.  The pair pass of the second evaluation writes its accelerations into
+// the spare set (acc_swap), so that the first evaluation's stay readable.  The one rule: whatever
+// could observe x .. rho or p / cs not being written yet -- reads or changes them, a full build, a
+// push, a change of the particle set, the stream or the time-control block, any stage but the
+// fused stage 2 -- runs half_materialise first; the fused stage 2 clears half_pending without it.
+static int half_materialise(b200sph_ctx *ctx)
+{
+    if (!ctx->half_pending) return 0;
+    ctx->half_pending = false;
+    StageArgs sa;
+    stage_args(ctx, sa, -1, 1, 0.0, false);
+    sa.f = ctx->half_f;
+    sa.tc = ctx->half_tc;
+    sa.rho = f64_ptr(ctx, B200SPH_RHO); sa.rho0 = f64_ptr(ctx, B200SPH_RHO0); sa.arho = f32_ptr(ctx, B200SPH_ARHO);
+    if (ctx->acc_swapped) {
+        sa.arho = ctx->acc_spare[0];
+        sa.au = ctx->acc_spare[1]; sa.av = ctx->acc_spare[2]; sa.aw = ctx->acc_spare[3];
+        sa.ax = ctx->acc_spare[4]; sa.ay = ctx->acc_spare[5]; sa.az = ctx->acc_spare[6];
+        ctx->acc_swapped = false;
+    }
+    if (ctx->pool_end > 0) {
+        k_half_materialise<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(
+            sa, f32_ptr(ctx, B200SPH_P), f32_ptr(ctx, B200SPH_CS), ctx->half_eos, ctx->half_EP);
+        LAUNCH_CHECK();
+    }
+    ctx->n_half_materialised++;
+    return 0;
+}
+
+// a deferred half step, then a deferred initialize (the two are never pending together)
+static int materialise_pending(b200sph_ctx *ctx)
+{
+    if (int rc = half_materialise(ctx)) return rc;
+    return init_materialise(ctx);
+}
+
+// The accelerations a pair pass writes, as ACC_* bits: au .. aw of array d (bit d), ax .. az
+// (bit 8 + d) and arho (bit 16 + d).  k_pair_list_r32 writes them exactly where the Group has a
+// momentum / an XSPH / a continuity equation for the destination's array; for the other pair
+// kernels the mask takes every array.
+enum { ACC_UVW = 0, ACC_XYZ = 8, ACC_RHO = 16 };
+static unsigned acc_writes(const b200sph_ctx *ctx, const b200sph_pair_program *prog, bool r32)
+{
+    if (!r32) return ~0u;
+    unsigned w = 0;
+    for (int d = 0; d < ctx->narr; d++) {
+        unsigned bits = 0;
+        for (int s = 0; s < ctx->narr; s++) bits |= prog->eqmask[d][s];
+        if (bits & B200SPH_EQ_MOMENTUM) w |= 1u << (ACC_UVW + d);
+        if (bits & B200SPH_EQ_XSPH) w |= 1u << (ACC_XYZ + d);
+        if (bits & B200SPH_EQ_CONTINUITY) w |= 1u << (ACC_RHO + d);
+    }
+    return w;
+}
+
+// The pair pass of the second evaluation (writes: acc_writes) while a half step is pending gets
+// the spare arho, au .. az: the two sets exchange names, as x / x0 do in init_by_rename, and the set of
+// the first evaluation stays in acc_spare for half_materialise.  A particle whose accelerations
+// this pass does not write must find the same values under the new names: where the sets may
+// differ there, the slots are copied into the spare set first (once, while the same passes run).
+static int acc_swap(b200sph_ctx *ctx, unsigned writes)
+{
+    const size_t n = (size_t)ctx->pool_cap;
+    for (Buf<float> &b : ctx->acc_spare)
+        if (int rc = grow(ctx, b, n, n)) return rc;
+    if (ctx->acc_differ & ~writes) {
+        for (int k = 0; k < 7; k++)
+            CU(cudaMemcpyAsync(ctx->acc_spare[k], ctx->prop[B200SPH_ARHO + k], sizeof(float) * (size_t)ctx->pool_end,
+                               cudaMemcpyDeviceToDevice, ctx->stream));
+        ctx->acc_differ = 0;
+    }
+    for (int k = 0; k < 7; k++) {
+        void *slot = ctx->prop[B200SPH_ARHO + k];
+        ctx->prop[B200SPH_ARHO + k] = ctx->acc_spare[k].p;
+        ctx->acc_spare[k].p = (float *)slot;
+    }
+    ctx->acc_swapped = true;
     return 0;
 }
 
@@ -1127,7 +1236,7 @@ const char *b200sph_last_error(b200sph_ctx *ctx)
 int b200sph_set_stream(b200sph_ctx *ctx, void *s)
 {
     CU(cudaSetDevice(ctx->device));
-    if (int rci = init_materialise(ctx)) return rci;
+    if (int rci = materialise_pending(ctx)) return rci;
     CU(cudaStreamSynchronize(ctx->stream));
     if (ctx->own_stream) CU(cudaStreamDestroy(ctx->stream));
     if (s) {
@@ -1153,7 +1262,7 @@ int b200sph_add_array(b200sph_ctx *ctx, const char *name, int64_t n, int64_t n_r
     if (ctx->narr >= B200SPH_MAX_ARRAYS) return set_err(ctx, "too many particle arrays (max %d)", B200SPH_MAX_ARRAYS);
     if (n < 0 || n_real < 0 || n_real > n) return set_err(ctx, "add_array: bad sizes n=%lld n_real=%lld", (long long)n, (long long)n_real);
     CU(cudaSetDevice(ctx->device));
-    if (int rci = init_materialise(ctx)) return rci;   // (before the layout moves)
+    if (int rci = materialise_pending(ctx)) return rci;   // (before the layout moves)
     const int a = ctx->narr;
     ctx->arr[a].name = name ? name : "";
     ctx->arr[a].n = n;
@@ -1179,7 +1288,7 @@ int b200sph_resize_array(b200sph_ctx *ctx, int arr, int64_t n, int64_t n_real)
     if (arr < 0 || arr >= ctx->narr) return set_err(ctx, "resize_array: bad array %d", arr);
     if (n < 0 || n_real < 0 || n_real > n) return set_err(ctx, "resize_array: bad sizes");
     CU(cudaSetDevice(ctx->device));
-    if (int rci = init_materialise(ctx)) return rci;
+    if (int rci = materialise_pending(ctx)) return rci;
     { int rc0 = eos_flush(ctx); if (rc0) return rc0; }
     if (ctx->pool_cap == 0) {
         ctx->arr[arr].cap = std::max(ctx->arr[arr].cap, n);
@@ -1509,7 +1618,8 @@ int b200sph_set_mirror(b200sph_ctx *ctx, const int mirror[3], double n_layers)
 int b200sph_update_domain(b200sph_ctx *ctx)
 {
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_pool(ctx);
+    // (only the periodic wrap reads the state; the rest is h)
+    int rc = ensure_pool(ctx, true, !(ctx->periodic[0] || ctx->periodic[1] || ctx->periodic[2]));
     if (rc) return rc;
     if (ctx->periodic[0] || ctx->periodic[1] || ctx->periodic[2]) {
         // _box_wrap_periodic, nnps_base.pyx:699-743 (part of DomainManager.update)
@@ -1590,6 +1700,7 @@ static bool retire_build(b200sph_ctx *ctx)
 // zeroed (0: the drift is added to what red_u32 holds)
 static int pack_positions_light(b200sph_ctx *ctx, int clear)
 {
+    if (int rc = half_materialise(ctx)) return rc;
     if (clear) CU(cudaMemsetAsync(ctx->red_u32, 0, clear * sizeof(unsigned), ctx->stream));
     k_pack_pos_light<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
         f64_ptr(ctx, B200SPH_X), f64_ptr(ctx, B200SPH_Y), f64_ptr(ctx, B200SPH_Z), f64_ptr(ctx, B200SPH_H), ctx->perm, ctx->skey,
@@ -1723,6 +1834,7 @@ int b200sph_nnps_update(b200sph_ctx *ctx)
         else if (ctx->evals_since_build >= 1.5 * lstar) ctx->skin = std::max(ctx->skin_min, ctx->skin * 0.75);
         else if (ctx->evals_since_build < lstar / 1.5) ctx->skin = std::min(ctx->skin_max, ctx->skin * 1.33);
     }
+    if ((rc = half_materialise(ctx))) return rc;   // the full build reads x, y, z
     ctx->skin_next = -1.0;
     ctx->evals_since_build = 0;
     lists_stale(ctx);
@@ -2005,7 +2117,7 @@ static int eos_flush(b200sph_ctx *ctx, cudaStream_t on_comm_stream)
     // this launch on the communication stream itself, behind the scatter
     if (!on_comm_stream)
         if (int rcj = sync_comm(ctx)) return rcj;
-    if (int rci = init_materialise(ctx)) return rci;   // (it copies the rho of before these calls)
+    if (int rci = materialise_pending(ctx)) return rci;   // (it copies the rho of before these calls)
     cudaStream_t s = on_comm_stream ? on_comm_stream : ctx->stream;
     if (int rcp = eos_pool_flush(ctx, s)) return rcp;   // (the older calls first)
     if (!ctx->eos_any) return 0;
@@ -2037,6 +2149,7 @@ static int ab_positions(b200sph_ctx *ctx)
 static int pack_state(b200sph_ctx *ctx)
 {
     if (int rc = ab_positions(ctx)) return rc;   // (k_pack_rec32 reads them)
+    if (int rc = half_materialise(ctx)) return rc;   // (the packers read u, v, w, p, cs)
     // the packers read the pool's rho and apply eos_pending to it (eos_flush's order: the
     // initialize, then the older calls)
     if (ctx->eos_any || ctx->eos_pool_any) {
@@ -2710,9 +2823,10 @@ int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_
     for (int d = 0; d < ctx->narr; d++)
         for (int sx = 0; sx < ctx->narr; sx++) prog_bits |= prog->eqmask[d][sx];
     const bool wcsph_only = !(prog_bits & ~(unsigned)PAIR_EQS_WCSPH) && !prog->tensile_correction;
-    // SummationDensity stores rho: a deferred initialize must have copied it before
+    // SummationDensity stores rho: a deferred initialize must have copied it before, and a
+    // pending half step formed it
     const bool writes_rho = (prog_bits & B200SPH_EQ_SUMMATION_DENSITY) != 0;
-    if (writes_rho && (rc = init_materialise(ctx))) return rc;
+    if (writes_rho && (rc = materialise_pending(ctx))) return rc;
     bool r32 = false;
     int ea = -1;
     if ((rc = records32(ctx, use_lists && !ranged && wcsph_only, &r32, &ea))) return rc;
@@ -2756,6 +2870,15 @@ int b200sph_pair_pass(b200sph_ctx *ctx, const b200sph_pair_program *prog, int64_
     if (!use_lists && (ctx->periodic[0] || ctx->periodic[1] || ctx->periodic[2]))
         return set_err(ctx, "periodic domains need the neighbour-list path (B200SPH_PAIR_KERNEL=list, < 2^26 particles)");
     if (use_lists && (rc = prepare_lists(ctx, want, "pair_pass: the lists cannot index the particles"))) return rc;
+    // the accelerations of the evaluation before a pending half step are still needed: this pass
+    // writes into the spare set, or (another pair kernel) the half step is formed now
+    const unsigned acc_w = acc_writes(ctx, prog, r32);
+    if (ctx->half_pending && !ctx->acc_swapped && acc_w) {
+        if (r32 && use_lists) rc = acc_swap(ctx, acc_w);
+        else rc = half_materialise(ctx);
+        if (rc) return rc;
+    }
+    ctx->acc_differ |= acc_w;
     PhaseTimer pt(ctx, 1);
 
     PairArgs pa;
@@ -3140,6 +3263,11 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
     int rc = stage_begin(ctx, rk3 ? "stage_rk3" : "stage", arr, which, devdt, last, true);
     if (rc) return rc;
     const bool fused = ctx->pool_end > 0 && can_fuse_stage(ctx, arr);
+    // a pending half step: only the fused stage 2 that follows it, with the same kind of dt, reads
+    // neither x .. w nor p / cs, and forms the predicted rho itself
+    const bool takes_half = ctx->half_pending && fused && which == 2 && !rk3 && ctx->rec32 &&
+                            (devdt ? ctx->tc : nullptr) == ctx->half_tc;
+    if (!takes_half && (rc = half_materialise(ctx))) return rc;
     // EOS calls issued since the last pair pass, or any before an initialize (which copies the
     // rho they clamp), go to the pool now; the pool side a pair pass left is the fused kernel's
     if ((which == 0 || !fused || ctx->eos_any) && (rc = eos_flush(ctx))) return rc;
@@ -3181,6 +3309,17 @@ static int stage_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devd
         q.E = ctx->eos_last;
         q.eos_pool = ctx->eos_pool_any ? 1 : 0;
         q.EP = ctx->eos_pool;
+        q.half_pending = (do_init == INIT_RENAMED && !rk3 && q.R) ? 1 : 0;
+        if (takes_half && ctx->half_pending) {   // (still pending: eos_flush above may have formed it)
+            q.arho_half = ctx->acc_swapped ? ctx->acc_spare[0].p : f32_ptr(ctx, B200SPH_ARHO);
+            q.f_half = ctx->half_f;
+        }
+        ctx->half_pending = q.half_pending != 0;   // (stage 2 clears it)
+        ctx->acc_swapped = false;
+        if (ctx->half_pending) {
+            ctx->half_f = sa.f, ctx->half_tc = sa.tc;
+            ctx->half_eos = q.eos_pool, ctx->half_EP = q.EP;
+        }
         ctx->init_pending = false;
         ctx->eos_pool_any = false;
         if (q.reduce_dt && !ctx->red_armed) {
@@ -3224,6 +3363,7 @@ int b200sph_stage_rk3_dev(b200sph_ctx *ctx, int arr, int which) { return stage_i
 int b200sph_time_control(b200sph_ctx *ctx, double *external_block8, double **dev_block)
 {
     CU(cudaSetDevice(ctx->device));
+    if (int rc = half_materialise(ctx)) return rc;   // (its factor may be dt in this block)
     if (external_block8) {
         CU(ctx->tc_own.reset());
         ctx->tc = external_block8;
@@ -3271,7 +3411,7 @@ int b200sph_dt_propose(b200sph_ctx *ctx, double cfl, int fixed_h)
 {
     if (int rcc = require_confirmed(ctx, "dt_propose")) return rcc;
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_pool(ctx);
+    int rc = ensure_pool(ctx, true, true);   // (dt_cfl, dt_force and h only)
     if (rc) return rc;
     if ((rc = b200sph_time_control(ctx, nullptr, nullptr))) return rc;
     PhaseTimer pt(ctx, 2);
@@ -3289,7 +3429,7 @@ int b200sph_dt_advance(b200sph_ctx *ctx, double cfl, int fixed_h, double prev_fa
 {
     if (int rcc = require_confirmed(ctx, "dt_advance")) return rcc;
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_pool(ctx);
+    int rc = ensure_pool(ctx, true, true);   // (dt_cfl, dt_force and h only)
     if (rc) return rc;
     if ((rc = b200sph_time_control(ctx, nullptr, nullptr))) return rc;
     if (!(prev_factor > 0.0) || !(new_factor > 0.0)) return set_err(ctx, "dt_advance: damping factors must be positive");
@@ -3359,7 +3499,7 @@ int b200sph_dt_factors(b200sph_ctx *ctx, double out[3])
 {
     if (int rcc = require_confirmed(ctx, "dt_factors")) return rcc;
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_pool(ctx);
+    int rc = ensure_pool(ctx, true, true);   // (dt_cfl, dt_force and h only)
     if (rc) return rc;
     PhaseTimer pt(ctx, 2);
     if ((rc = reduce_dt_factors(ctx))) return rc;
@@ -4037,7 +4177,7 @@ int b200sph_drop_ghosts(b200sph_ctx *ctx, int arr)
     if (arr < 0 || arr >= ctx->narr) return set_err(ctx, "drop_ghosts: bad array %d", arr);
     if (ctx->arr[arr].n != ctx->arr[arr].n_real) {
         CU(cudaSetDevice(ctx->device));
-        if (int rci = init_materialise(ctx)) return rci;
+        if (int rci = materialise_pending(ctx)) return rci;
         ctx->arr[arr].n = ctx->arr[arr].n_real;
         set_changed(ctx);
     }
@@ -4198,6 +4338,12 @@ int b200sph_reset_stats(b200sph_ctx *ctx)
     b200sph_get_stats(ctx, &tmp);  // drain pending events
     memset(&ctx->stats, 0, sizeof(ctx->stats));
     ctx->n_full_builds = ctx->n_light_updates = ctx->n_list_builds = ctx->n_deferred_failed = ctx->n_fused = ctx->n_overlapped = ctx->n_proactive = ctx->n_pair_r32 = 0;
+    ctx->n_half_materialised = 0;
+    return 0;
+}
+int b200sph_half_materialised(b200sph_ctx *ctx, int64_t *out)
+{
+    *out = ctx->n_half_materialised;
     return 0;
 }
 int b200sph_records32_launches(b200sph_ctx *ctx, int64_t *out)

@@ -290,6 +290,11 @@ struct FusePackArgs {
     EosTab E;
     int eos_pool;                    // apply EP to the pool's rho / p / cs first
     EosTab EP;
+    int half_pending;                // WCSPHStep stage 1: x .. rho and EP's p / cs are left to half_materialise
+    // WCSPHStep stage 2 after such a stage 1: the predicted rho its EOS calls read is formed again
+    // from rho0, stage 1's factor f_half and the first evaluation's arho (arho_half), as stage 1 did
+    const float *arho_half;
+    double f_half;
 };
 
 // The body of the fused stage kernels, the stage being WCSPHStep's or, RK3, WCSPHTVDRK3Step's.
@@ -330,12 +335,19 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
                 r0 = a.rho0[g];
             }
             double rc = r0;
-            if (q.do_init == INIT_NONE && (eos || (RK3 && a.which != 1))) rc = a.rho[g];
+            if (!RK3 && q.arho_half) {
+                if (eos) rc = wcsph_combine(r0, stage_factor(a.tc, q.f_half, 1, false), q.arho_half[g]);
+            } else if (q.do_init == INIT_NONE && (eos || (RK3 && a.which != 1))) {
+                rc = a.rho[g];
+            }
             float p_eos = 0.f, cs_eos = 0.f;
+            const bool store = RK3 || !q.half_pending;
             if (eos) {
                 eos_tab_eval(q.EP, t & 7, rc, p_eos, cs_eos);
-                q.p[g] = p_eos;
-                q.cs[g] = cs_eos;
+                if (store) {
+                    q.p[g] = p_eos;
+                    q.cs[g] = cs_eos;
+                }
             }
             double un, vn, wn, xn, yn, zn, r;
             if (RK3) {
@@ -355,9 +367,11 @@ __device__ __forceinline__ void stage_pack_body(const StageArgs &a, const FusePa
                 zn = wcsph_combine(z0, f, a.az[g]);
                 r = wcsph_combine(r0, f, a.arho[g]);
             }
-            a.u[g] = un; a.v[g] = vn; a.w[g] = wn;
-            a.x[g] = xn; a.y[g] = yn; a.z[g] = zn;
-            a.rho[g] = r;
+            if (store) {
+                a.u[g] = un; a.v[g] = vn; a.w[g] = wn;
+                a.x[g] = xn; a.y[g] = yn; a.z[g] = zn;
+                a.rho[g] = r;
+            }
             if (q.reduce_dt) {
                 mc = (double)q.dt_cfl[g];
                 mf = (double)q.dt_force[g];
@@ -443,6 +457,33 @@ __global__ void __launch_bounds__(256, 4) k_stage_pack_rk3(const StageArgs a, co
     __shared__ float s_d2[8], s_dh[8];
     __shared__ double s_mc[8], s_mf[8], s_hm[8];
     stage_pack_body<true>(a, q, s_d2, s_dh, s_mc, s_mf, s_hm);
+}
+
+// What a fused stage 1 with half_pending left unwritten, from the operands that stage read: x .. rho
+// = wcsph_combine(x0 .. rho0, f, ax .. arho) with a.au .. a.arho the FIRST evaluation's
+// accelerations (the pair pass of the second one writes into the spare set) and the stage's
+// factor, and p, cs = the pool side of EP on rho0 (with INIT_RENAMED the stage's rho before the
+// EOS calls is rho0).  The same functions on the same doubles: bitwise what the stage would have
+// stored.
+__global__ void k_half_materialise(const StageArgs a, float *__restrict__ p, float *__restrict__ cs, const int eos_pool,
+                                   const EosTab EP)
+{
+    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= a.pool_end) return;
+    const uint8_t t = a.ptype[g];
+    if (t == PT_INVALID || (t & PT_GHOST)) return;
+    const double f = stage_factor(a.tc, a.f, 1, false);
+    a.u[g] = wcsph_combine(a.u0[g], f, a.au[g]);
+    a.v[g] = wcsph_combine(a.v0[g], f, a.av[g]);
+    a.w[g] = wcsph_combine(a.w0[g], f, a.aw[g]);
+    a.x[g] = wcsph_combine(a.x0[g], f, a.ax[g]);
+    a.y[g] = wcsph_combine(a.y0[g], f, a.ay[g]);
+    a.z[g] = wcsph_combine(a.z0[g], f, a.az[g]);
+    a.rho[g] = wcsph_combine(a.rho0[g], f, a.arho[g]);
+    if (eos_pool && eos_tab_applies(EP, t)) {
+        double rc = a.rho0[g];
+        eos_tab_eval(EP, t & 7, rc, p[g], cs[g]);
+    }
 }
 
 __global__ void k_eos_tab(double *__restrict__ rho, float *__restrict__ p, float *__restrict__ cs,
