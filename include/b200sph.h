@@ -74,6 +74,15 @@ enum {
     B200SPH_R00 = 91, B200SPH_R01, B200SPH_R02, B200SPH_R11, B200SPH_R12, B200SPH_R22,
     B200SPH_AS00 = 97, B200SPH_AS01, B200SPH_AS02, B200SPH_AS11, B200SPH_AS12, B200SPH_AS22,
     B200SPH_SOLID_PROPS_END = 103,
+    /* implicit incompressible SPH extension (get_particle_array_iisph, pysph/base/utils.py:
+     * 193-236), fp64, device memory allocated as one group on first use: ids 140 .. 153, above
+     * the user properties.  An IISPH array keeps its pressure p (the warm start of the next
+     * pressure solve) in the fp64 B200SPH_PF and p0 in B200SPH_PF0, and its V (the solids'
+     * number density) in B200SPH_IISPH_V. */
+    B200SPH_UADV = 140, B200SPH_VADV, B200SPH_WADV, B200SPH_RHO_ADV,
+    B200SPH_DII0 = 144, B200SPH_DII1, B200SPH_DII2, B200SPH_AII,
+    B200SPH_DIJPJ0 = 148, B200SPH_DIJPJ1, B200SPH_DIJPJ2, B200SPH_PITER,
+    B200SPH_COMPRESSION = 152, B200SPH_IISPH_V = 153,
     /* 32-bit integer props */
     B200SPH_GID = 64, B200SPH_TAG = 65, B200SPH_PID = 66,
     /* fp64 properties the pool does not know, created on first use for the generic-equation
@@ -143,6 +152,25 @@ typedef struct {
     int32_t clamp_p;     /* ClampWallPressure (wc/edac.py:169-174) on the walls   */
     double eps_xsph;     /* XSPHCorrection(eps) of the external-flow branch       */
 } b200sph_tvf_program;
+
+/* The Groups of IISPHScheme.get_equations (pysph/sph/iisph.py:511-643) in one call: NumberDensity
+ * of the solids, SummationDensity(+Boundary), AdvectionAcceleration + ComputeDII(+Boundary) +
+ * ViscosityAcceleration(+Boundary) (nu > 0), ComputeRhoAdvection + ComputeAII(+Boundary), the
+ * pressure iterations Group(iterate=True, min_iterations, max_iterations) of ComputeDIJPJ and
+ * PressureSolve(+Boundary), and PressureForce(+Boundary).  Every fluid is a destination and a
+ * source of the fluid equations; every solid a source of the boundary equations. */
+typedef struct {
+    uint32_t fluid_mask;   /* bit a: array a is a fluid                                 */
+    uint32_t solid_mask;   /* bit a: array a is a solid (0: none)                       */
+    double rho0, nu;
+    double gx, gy, gz;
+    double omega, tolerance;
+    int32_t min_iterations, max_iterations;
+    double dt;             /* the evaluation's dt (AdvectionAcceleration, ComputeRhoAdvection,
+                            * PressureSolve read it) ...                                */
+    int32_t dt_device;     /* ... or, != 0, dt from the device time-control block       */
+    int32_t reserved;
+} b200sph_iisph_program;
 
 /* The two Groups of ElasticSolidsScheme.get_equations (solid_mech/basic.py:604-651) for
  * elastic solids (destinations and sources) and rigid `solids` (sources only).  Group 1: IsothermalEOS (:93-101), VelocityGradient2D/3D
@@ -430,6 +458,20 @@ int b200sph_stage_tvf_dev(b200sph_ctx *ctx, int arr, int which);
  * as stage_tvf, but positions move with the XSPH-corrected velocity ax ay az */
 int b200sph_stage_edac(b200sph_ctx *ctx, int arr, int which, double dt);
 int b200sph_stage_edac_dev(b200sph_ctx *ctx, int arr, int which);
+
+/* The IISPH evaluation (see b200sph_iisph_program), on the persistent neighbour lists.  The host
+ * enqueues max_iterations pressure iterations and never waits: the device decides after each
+ * one whether the iterations are over, and the iterations after that return at once.  When
+ * the evaluation repeats after a failed deferred drift check (b200sph_nnps_confirm), the repeat
+ * starts from the pressure the first attempt started from (p = p0).  Refused: the slab
+ * decomposition, mirror domains, ghost particles, 1-D.  pairs_out may be NULL. */
+int b200sph_iisph_pass(b200sph_ctx *ctx, const b200sph_iisph_program *prog, int64_t *pairs_out);
+/* the last IISPH evaluation: *iterations run and PressureSolve.compression (|avg - rho0| / rho0)
+ * of every array after the last one (0 for the arrays that are no fluid); waits */
+int b200sph_iisph_stats(b200sph_ctx *ctx, int *iterations, double compression[B200SPH_MAX_ARRAYS]);
+/* IISPHStep.stage1 (iisph.py:22-34): u = uadv + dt au, x += dt u (which must be 1) */
+int b200sph_stage_iisph(b200sph_ctx *ctx, int arr, int which, double dt);
+int b200sph_stage_iisph_dev(b200sph_ctx *ctx, int arr, int which);
 
 /* The elastic-dynamics evaluation (see b200sph_solid_program); same neighbour lists as
  * pair_pass. */

@@ -9,11 +9,12 @@ reference (pypr/pysph)      here
 ==========================  ==================================================
 compiled AccelerationEval   :class:`B200AccelerationEval`
 compiled Integrator         :class:`PECIntegrator`, :class:`EPECIntegrator`,
-                            :class:`TVDRK3Integrator`
+                            :class:`TVDRK3Integrator`, :class:`EulerIntegrator`
 NNPS (LinkedListNNPS)       :class:`B200NNPS`
 DeviceHelper (``pa.gpu``)   :class:`B200DeviceHelper` / :class:`B200Backend`
 Equation / Group            :mod:`pysph_b200.equations`
 WCSPHScheme.get_equations   :class:`pysph_b200.scheme.WCSPHScheme`
+IISPHScheme.get_equations   :class:`pysph_b200.iisph.IISPHScheme`
 Solver step loop            :class:`B200Solver`
 solver tools                :class:`DensityCorrection`, :class:`ShiftPositions`
 tools.interpolator          :class:`Interpolator`
@@ -39,7 +40,7 @@ from .domain import DomainManager
 from .nnps import B200NNPS
 from .acceleration_eval import B200AccelerationEval
 from .integrator import (B200Integrator, PECIntegrator, EPECIntegrator,
-                         TVDRK3Integrator, WCSPHStep, WCSPHTVDRK3Step)
+                         TVDRK3Integrator, EulerIntegrator, WCSPHStep, WCSPHTVDRK3Step)
 from .solver import B200Solver
 from .tools import Tool, DensityCorrection
 from .shift import SimpleShift, FickianShift, CorrectVelocities, ShiftPositions
@@ -47,6 +48,8 @@ from .interpolator import Interpolator, get_bounding_box, get_nx_ny_nz
 from .edac import EDACScheme, EDACTVFStep, EDACStep
 from .output import dump, load
 from .solid_mech import ElasticSolidsScheme, SolidMechStep
+from .iisph import (IISPHScheme, IISPHStep, get_particle_array_iisph, make_iisph_solver,
+                    last_iterations)
 
 __version__ = '0.1.0'
 

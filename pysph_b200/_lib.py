@@ -39,6 +39,12 @@ ELASTIC_PROP_IDS.update(('s' + k + '0', 76 + i) for i, k in enumerate(_SYM))
 ELASTIC_PROP_IDS.update(('v%d%d' % (i, j), 82 + 3 * i + j) for i in range(3) for j in range(3))
 ELASTIC_PROP_IDS.update(('r' + k, 91 + i) for i, k in enumerate(_SYM))
 ELASTIC_PROP_IDS.update(('as' + k, 97 + i) for i, k in enumerate(_SYM))
+# implicit incompressible SPH extension (B200SPH_UADV ...); arrays that own 'uadv' use these.
+# p (the pressure solve's warm start) and p0 live in the fp64 B200SPH_PF / B200SPH_PF0, V in fp64
+IISPH_PROP_IDS = dict(PROP_IDS, p=30, p0=31, V=153)
+IISPH_PROP_IDS.update((n, 140 + i) for i, n in enumerate(
+    ('uadv', 'vadv', 'wadv', 'rho_adv', 'dii0', 'dii1', 'dii2', 'aii', 'dijpj0', 'dijpj1',
+     'dijpj2', 'piter', 'compression')))
 INT_PROP_IDS = {'gid': 64, 'tag': 65, 'pid': 66}
 USER_PROP0, MAX_USER_PROPS = 110, 16     # B200SPH_USER0, B200SPH_MAX_USER
 F64_DEVICE_PROPS = ('x', 'y', 'z', 'u', 'v', 'w', 'rho', 'h', 'm',
@@ -97,6 +103,15 @@ class SolidProgram(C.Structure):
                 ('wdeltap', C.c_double * MAX_ARRAYS), ('n', C.c_double * MAX_ARRAYS),
                 ('G', C.c_double * MAX_ARRAYS),
                 ('source_mask', C.c_uint32), ('reserved', C.c_uint32)]
+
+
+class IisphProgram(C.Structure):
+    _fields_ = [('fluid_mask', C.c_uint32), ('solid_mask', C.c_uint32),
+                ('rho0', C.c_double), ('nu', C.c_double),
+                ('gx', C.c_double), ('gy', C.c_double), ('gz', C.c_double),
+                ('omega', C.c_double), ('tolerance', C.c_double),
+                ('min_iterations', C.c_int32), ('max_iterations', C.c_int32),
+                ('dt', C.c_double), ('dt_device', C.c_int32), ('reserved', C.c_int32)]
 
 
 class GridInfo(C.Structure):
@@ -180,6 +195,10 @@ SIGNATURES = {
     'b200sph_solid_pass': (C.c_int, [_ctx_p, C.POINTER(SolidProgram), C.POINTER(_i64)]),
     'b200sph_stage_solid': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_double]),
     'b200sph_stage_solid_dev': (C.c_int, [_ctx_p, C.c_int, C.c_int]),
+    'b200sph_iisph_pass': (C.c_int, [_ctx_p, C.POINTER(IisphProgram), C.POINTER(_i64)]),
+    'b200sph_iisph_stats': (C.c_int, [_ctx_p, C.POINTER(C.c_int), _dp]),
+    'b200sph_stage_iisph': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_double]),
+    'b200sph_stage_iisph_dev': (C.c_int, [_ctx_p, C.c_int, C.c_int]),
     'b200sph_stage': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_double]),
     'b200sph_dt_factors': (C.c_int, [_ctx_p, _dp]),
     'b200sph_time_control': (C.c_int, [_ctx_p, C.c_void_p, C.POINTER(C.c_void_p)]),

@@ -62,6 +62,13 @@ class B200AccelerationEval(object):
         self.nnps = None
         self.count_pairs = False
         self.last_pairs = 0
+        # the integrator's: dt of compute(t, dt) is the device-resident one (the IISPH op reads
+        # it on the device, so that host-dt and device-dt runs stay bitwise equal)
+        self.device_dt = False
+        self.iisph_fluids = ()
+        for op in self.ops:
+            if op[0] == 'iisph':
+                self.iisph_fluids = op[2]
         # reference API: AccelerationEval.c_acceleration_eval is "the compiled
         # object"; here the adapter is its own compiled object
         self.c_acceleration_eval = self
@@ -151,6 +158,12 @@ class B200AccelerationEval(object):
                 self._pairs += cnt.value if self.count_pairs else 0
             elif kind == 'correct_vel':
                 ctx.call('b200sph_correct_velocities', op[1], C.byref(cnt) if self.count_pairs else None)
+                self._pairs += cnt.value if self.count_pairs else 0
+            elif kind == 'iisph':
+                prog = op[1]
+                prog.dt = float(dt)
+                prog.dt_device = 1 if self.device_dt else 0
+                ctx.call('b200sph_iisph_pass', C.byref(prog), C.byref(cnt) if self.count_pairs else None)
                 self._pairs += cnt.value if self.count_pairs else 0
             elif kind == 'update_nnps':
                 # mako:139-145: nnps.update_domain(); nnps.update()

@@ -22,7 +22,7 @@
 // One translation unit: this file holds the context, the pool and every C-ABI entry
 // point; the kernels are included below by family (pool_kernels, scan, nnps_kernels,
 // sph_kernels, pair_kernel, pair_list, tvf_kernels, solid_kernels, halo_kernels, density_filter,
-// interp_kernels, shift_kernels .cuh).
+// interp_kernels, shift_kernels, iisph_kernels .cuh).
 //
 // No CPU fallback: every entry point needs a CUDA device.
 #include "b200sph.h"
@@ -45,7 +45,7 @@
 // --------------------------------------------------------------------------
 // small helpers
 // --------------------------------------------------------------------------
-#define N_PROP_SLOTS (B200SPH_USER0 + B200SPH_MAX_USER)   // property ids 0 .. the last user property
+#define N_PROP_SLOTS (B200SPH_IISPH_V + 1)   // property ids 0 .. the last IISPH property
 #define PT_INVALID 0xFFu
 #define PT_GHOST 0x08u
 
@@ -246,6 +246,7 @@ template <class T, Mem M = Mem::DEVICE> struct Buf {
 struct PeerBox;
 struct PeerDecision;
 struct ShiftRec;    // shift_kernels.cuh
+struct IisphState;  // iisph_kernels.cuh
 
 struct b200sph_ctx {
     int device = 0;
@@ -424,6 +425,14 @@ struct b200sph_ctx {
     Buf<double> shift_dpos, shift_dvel;
     Buf<long long> shift_vmax;
     unsigned shift_mask = 0;
+    // implicit incompressible SPH (b200sph_iisph_pass): the position records [n_sorted], the new
+    // pressure of an iteration [pool_end], the partial sums of its reduction and the iteration
+    // state.  iisph_spec: an IISPH evaluation ran on a deferred drift check not yet confirmed;
+    // iisph_restore: that check failed, so the repeat starts from p = p0 (the step's pressure)
+    Buf<ShiftRec> iisph_P;
+    Buf<double> iisph_pnext, iisph_part;
+    Buf<IisphState> iisph_st;
+    bool iisph_spec = false, iisph_restore = false;
     // Group(start_idx, stop_idx): one-shot destination ranges of the next pair pass
     int64_t dst_lo[B200SPH_MAX_ARRAYS] = {0}, dst_hi[B200SPH_MAX_ARRAYS] = {0};
     bool dst_ranged = false;
@@ -708,16 +717,18 @@ __device__ __forceinline__ void rec32_make(const float4 A, const double u, const
 #include "density_filter.cuh"
 #include "interp_kernels.cuh"
 #include "shift_kernels.cuh"
+#include "iisph_kernels.cuh"
 
 // --------------------------------------------------------------------------
 // host side
 // --------------------------------------------------------------------------
 // What a property id of the header's enum is: its element type on the device (PROP_NONE: no such
 // property) and when its buffer is allocated -- with the pool, as a group the first time any
-// elastic-dynamics property is named (with the stress records T01 T2R R2), or one by one when a
+// elastic-dynamics property is named (with the stress records T01 T2R R2), as a group the first
+// time any IISPH property is named, or one by one when a
 // user property is named.  The only host code that knows the ranges of the id enum.
 enum PropType { PROP_NONE, PROP_F64, PROP_F32, PROP_U32 };
-enum PropGroup { GROUP_POOL, GROUP_ELASTIC, GROUP_USER };
+enum PropGroup { GROUP_POOL, GROUP_ELASTIC, GROUP_IISPH, GROUP_USER };
 struct PropKind {
     PropType type;
     PropGroup group;
@@ -732,6 +743,7 @@ static PropKind prop_kind(int p)
     if (p >= B200SPH_GID && p <= B200SPH_PID) return {PROP_U32, GROUP_POOL};
     if (p >= B200SPH_S00 && p <= B200SPH_S220) return {PROP_F64, GROUP_ELASTIC};
     if (p >= B200SPH_V00 && p <= B200SPH_AS22) return {PROP_F32, GROUP_ELASTIC};
+    if (p >= B200SPH_UADV && p <= B200SPH_IISPH_V) return {PROP_F64, GROUP_IISPH};
     if (p >= B200SPH_USER0 && p < B200SPH_USER0 + B200SPH_MAX_USER) return {PROP_F64, GROUP_USER};
     return {PROP_NONE, GROUP_POOL};
 }
@@ -1757,7 +1769,9 @@ static int confirm_pending(b200sph_ctx *ctx, int *redo)
         ctx->n_light_updates--;
         ctx->n_deferred_failed++;
         *redo = 1;
+        ctx->iisph_restore = ctx->iisph_spec;
     }
+    ctx->iisph_spec = false;
     return 0;
 }
 // entry points that consume the results of an evaluation must not run on an
@@ -3242,6 +3256,190 @@ static int ensure_tc(b200sph_ctx *ctx)
     CU(cudaMemcpy(ctx->tc, init, sizeof(init), cudaMemcpyHostToDevice));
     return 0;
 }
+
+// ---- implicit incompressible SPH (iisph_kernels.cuh) -----------------------------------------
+// A list consumer of the evaluation, like the EDAC and elastic-dynamics passes: it may run on a
+// deferred drift check that the caller confirms afterwards (the evaluation is then repeated), so
+// it does not wait for that check itself.  Everything it writes is overwritten by a repeat but
+// the pressure, the warm start of the next solve: a repeat starts from p = p0 again.
+int b200sph_iisph_pass(b200sph_ctx *ctx, const b200sph_iisph_program *prog, int64_t *pairs_out)
+{
+    CU(cudaSetDevice(ctx->device));
+    int rc = ensure_pool(ctx);
+    if (rc) return rc;
+    const unsigned fm = prog->fluid_mask, sm = prog->solid_mask;
+    if (fm == 0 || fm >= (1u << ctx->narr)) return set_err(ctx, "iisph_pass: bad fluid mask 0x%x", fm);
+    if (sm >= (1u << ctx->narr) || (sm & fm)) return set_err(ctx, "iisph_pass: bad solid mask 0x%x (fluids 0x%x)", sm, fm);
+    if (prog->min_iterations < 0 || prog->max_iterations < 1)
+        return set_err(ctx, "iisph_pass: iterations must be min >= 0, max >= 1 (got %d, %d)", prog->min_iterations, prog->max_iterations);
+    if (ctx->dim < 2) return set_err(ctx, "iisph_pass: IISPH runs in 2-D and 3-D");
+    if (ctx->peer_box || ctx->comm_pending) return set_err(ctx, "iisph_pass runs on one GPU (no slab decomposition)");
+    if (mirror_any(ctx)) return set_err(ctx, "iisph_pass: mirror domains are not supported");
+    for (int a = 0; a < ctx->narr; a++)
+        if (ctx->arr[a].n != ctx->arr[a].n_real)
+            return set_err(ctx, "iisph_pass: array '%s' has ghost particles (the pressure iterations do not refresh them)", ctx->arr[a].name.c_str());
+    if (!ctx->grid_valid) return set_err(ctx, "iisph_pass: the NNPS is stale (particles were pushed, resized or moved); call nnps_update first");
+    if ((rc = ensure_prop(ctx, B200SPH_UADV))) return rc;
+    if ((rc = eos_flush(ctx)) || (rc = ab_positions(ctx))) return rc;
+    if (prog->dt_device && (rc = ensure_tc(ctx))) return rc;
+    if ((rc = grow(ctx, ctx->iisph_st, 1, 1))) return rc;
+    if (ctx->iisph_restore) {
+        // the first attempt of this evaluation solved p from p0: start again from there
+        for (int a = 0; a < ctx->narr; a++)
+            if (((fm >> a) & 1u) && ctx->arr[a].n > 0)
+                CU(cudaMemcpyAsync(f64_ptr(ctx, B200SPH_PF) + ctx->arr[a].off, f64_ptr(ctx, B200SPH_PF0) + ctx->arr[a].off,
+                                   8 * (size_t)ctx->arr[a].n, cudaMemcpyDeviceToDevice, ctx->stream));
+        ctx->iisph_restore = false;
+    }
+    ctx->iisph_spec = ctx->check_pending;
+    CU(cudaMemsetAsync(ctx->iisph_st, 0, sizeof(IisphState), ctx->stream));
+    if (ctx->n_sorted == 0) {
+        if (pairs_out) *pairs_out = 0;
+        return 0;
+    }
+    unsigned long long want[B200SPH_MAX_ARRAYS] = {0};
+    for (int a = 0; a < ctx->narr; a++) {
+        if ((fm >> a) & 1u)
+            for (int b = 0; b < ctx->narr; b++)
+                if (((fm | sm) >> b) & 1u) want[a] |= 0xFFull << (8 * b);
+        if ((sm >> a) & 1u) want[a] |= 0xFFull << (8 * a);
+    }
+    if ((rc = prepare_lists(ctx, want, "iisph_pass: the neighbour lists cannot index the particles"))) return rc;
+    const size_t n = (size_t)ctx->n_sorted, np = (size_t)ctx->pool_end;
+    int64_t nmax = 1;
+    for (int a = 0; a < ctx->narr; a++) nmax = std::max<int64_t>(nmax, ctx->arr[a].n);
+    const size_t nbr = (size_t)cdiv(nmax, IISPH_RED);
+    if ((rc = grow(ctx, ctx->iisph_P, n, n)) || (rc = grow(ctx, ctx->iisph_pnext, np, np)) ||
+        (rc = grow(ctx, ctx->iisph_part, 2 * nbr, 2 * nbr)))
+        return rc;
+    IisphArgs ia;
+    memset(&ia, 0, sizeof(ia));
+    ia.P = ctx->iisph_P;
+    ia.perm = ctx->perm; ia.cnt = ctx->cnt; ia.lst = ctx->lst; ia.skey = ctx->skey; ia.stype = ctx->stype;
+    ia.x = f64_ptr(ctx, B200SPH_X); ia.y = f64_ptr(ctx, B200SPH_Y); ia.z = f64_ptr(ctx, B200SPH_Z);
+    ia.h = f64_ptr(ctx, B200SPH_H); ia.m = f64_ptr(ctx, B200SPH_M);
+    ia.rho = f64_ptr(ctx, B200SPH_RHO); ia.rho_c = ia.rho;
+    ia.u = f64_ptr(ctx, B200SPH_U); ia.v = f64_ptr(ctx, B200SPH_V); ia.w = f64_ptr(ctx, B200SPH_W);
+    ia.V = f64_ptr(ctx, B200SPH_IISPH_V);
+    ia.uadv = f64_ptr(ctx, B200SPH_UADV); ia.vadv = f64_ptr(ctx, B200SPH_VADV); ia.wadv = f64_ptr(ctx, B200SPH_WADV);
+    ia.rho_adv = f64_ptr(ctx, B200SPH_RHO_ADV);
+    ia.dii0 = f64_ptr(ctx, B200SPH_DII0); ia.dii1 = f64_ptr(ctx, B200SPH_DII1); ia.dii2 = f64_ptr(ctx, B200SPH_DII2);
+    ia.aii = f64_ptr(ctx, B200SPH_AII);
+    ia.dijpj0 = f64_ptr(ctx, B200SPH_DIJPJ0); ia.dijpj1 = f64_ptr(ctx, B200SPH_DIJPJ1); ia.dijpj2 = f64_ptr(ctx, B200SPH_DIJPJ2);
+    ia.p = f64_ptr(ctx, B200SPH_PF); ia.p0 = f64_ptr(ctx, B200SPH_PF0);
+    ia.piter = f64_ptr(ctx, B200SPH_PITER); ia.pnext = ctx->iisph_pnext; ia.comp = f64_ptr(ctx, B200SPH_COMPRESSION);
+    ia.au = f32_ptr(ctx, B200SPH_AU); ia.av = f32_ptr(ctx, B200SPH_AV); ia.aw = f32_ptr(ctx, B200SPH_AW);
+    ia.dt_cfl = f32_ptr(ctx, B200SPH_DT_CFL); ia.dt_force = f32_ptr(ctx, B200SPH_DT_FORCE);
+    ia.st = ctx->iisph_st; ia.part = ctx->iisph_part;
+    ia.n = ctx->n_sorted; ia.capg = ctx->capg;
+    ia.ncx = ctx->G.nc[0]; ia.ncy = ctx->G.nc[1]; ia.zorder = ctx->G.zorder;
+    for (int d = 0; d < 3; d++) {
+        ia.per[d] = ctx->G.periodic[d];
+        ia.L[d] = ctx->dom_hi[d] - ctx->dom_lo[d];
+    }
+    ia.kr = ctx->radius_scale;
+    ia.kfac = kernel_fac(ctx->kernel, ctx->dim);
+    ia.fluid_mask = fm; ia.solid_mask = sm;
+    ia.rho0 = prog->rho0; ia.nu = prog->nu; ia.gx = prog->gx; ia.gy = prog->gy; ia.gz = prog->gz;
+    ia.omega = prog->omega; ia.tol = prog->tolerance;
+    ia.min_it = prog->min_iterations; ia.max_it = prog->max_iterations;
+    ia.dt = prog->dt; ia.tc = prog->dt_device ? ctx->tc : nullptr;
+    if ((rc = pairs_arm(ctx, pairs_out, &ia.pair_counter))) return rc;
+    PhaseTimer pt(ctx, 2);
+    k_iisph_pack<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(ia);
+    LAUNCH_CHECK();
+    const unsigned nb = (unsigned)cdiv(ctx->n_sorted, IISPH_NT);
+    const auto pass = [&](const int which) {
+        return with_kernel_dim(ctx, "iisph_pass", [&](auto kc, auto dc) {
+            constexpr int K = decltype(kc)::value, D = decltype(dc)::value;
+            switch (which) {
+            case IISPH_V: k_iisph<K, D, IISPH_V><<<nb, IISPH_NT, 0, ctx->stream>>>(ia); break;
+            case IISPH_RHO: k_iisph<K, D, IISPH_RHO><<<nb, IISPH_NT, 0, ctx->stream>>>(ia); break;
+            case IISPH_ADV: k_iisph<K, D, IISPH_ADV><<<nb, IISPH_NT, 0, ctx->stream>>>(ia); break;
+            case IISPH_AII: k_iisph<K, D, IISPH_AII><<<nb, IISPH_NT, 0, ctx->stream>>>(ia); break;
+            case IISPH_DIJPJ: k_iisph<K, D, IISPH_DIJPJ><<<nb, IISPH_NT, 0, ctx->stream>>>(ia); break;
+            case IISPH_SOLVE: k_iisph<K, D, IISPH_SOLVE><<<nb, IISPH_NT, 0, ctx->stream>>>(ia); break;
+            default: k_iisph<K, D, IISPH_FORCE><<<nb, IISPH_NT, 0, ctx->stream>>>(ia); break;
+            }
+            LAUNCH_CHECK();
+            return 0;
+        });
+    };
+    if (sm && (rc = pass(IISPH_V))) return rc;
+    if ((rc = pass(IISPH_RHO)) || (rc = pass(IISPH_ADV)) || (rc = pass(IISPH_AII))) return rc;
+    int last = 0;
+    for (int a = 0; a < ctx->narr; a++)
+        if ((fm >> a) & 1u) last = a;
+    pt.to(1);
+    for (int it = 0; it < prog->max_iterations; it++) {
+        if ((rc = pass(IISPH_DIJPJ))) return rc;
+        for (int a = 0; a < ctx->narr; a++) {
+            if (!((fm >> a) & 1u)) continue;
+            ia.dest_mask = 1u << a;
+            if ((rc = pass(IISPH_SOLVE))) return rc;
+            if (ctx->arr[a].n > 0) {
+                k_iisph_commit<<<(unsigned)cdiv(ctx->arr[a].n, 256), 256, 0, ctx->stream>>>(ia, ctx->arr[a].off, ctx->arr[a].n);
+                LAUNCH_CHECK();
+            }
+        }
+        for (int a = 0; a < ctx->narr; a++) {
+            if (!((fm >> a) & 1u)) continue;
+            const long long nba = std::max<long long>(1, cdiv(ctx->arr[a].n, IISPH_RED));
+            if (ctx->arr[a].n > 0) {
+                k_iisph_partials<<<(unsigned)nba, IISPH_RED, 0, ctx->stream>>>(ia, ctx->arr[a].off, ctx->arr[a].n);
+                LAUNCH_CHECK();
+            }
+            k_iisph_converge<<<1, IISPH_RED, 0, ctx->stream>>>(ia, ctx->arr[a].n > 0 ? nba : 0, a, a == last);
+            LAUNCH_CHECK();
+        }
+        ctx->stats.pair_launches++;
+    }
+    if ((rc = pass(IISPH_FORCE))) return rc;
+    pt.stop();
+    // rho, p and the accelerations changed: the next evaluation packs its records from the pool
+    state_changed(ctx);
+    ctx->spec_records = false;
+    return pairs_read(ctx, pairs_out);
+}
+
+int b200sph_iisph_stats(b200sph_ctx *ctx, int *iterations, double compression[B200SPH_MAX_ARRAYS])
+{
+    CU(cudaSetDevice(ctx->device));
+    if (!ctx->iisph_st) return set_err(ctx, "iisph_stats: no IISPH evaluation has run");
+    IisphState st;
+    CU(cudaMemcpyAsync(&st, ctx->iisph_st, sizeof(st), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    *iterations = st.it;
+    for (int a = 0; a < B200SPH_MAX_ARRAYS; a++) compression[a] = st.comp[a];
+    return 0;
+}
+
+static int stage_iisph_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devdt)
+{
+    int rc = stage_begin(ctx, "stage_iisph", arr, which, devdt);
+    if (rc) return rc;
+    if (which != 1) return set_err(ctx, "stage_iisph: IISPHStep has stage1 only (which = 1, got %d)", which);
+    if ((rc = ensure_prop(ctx, B200SPH_UADV))) return rc;
+    PhaseTimer pt(ctx, 2);
+    StageIisphArgs sa;
+    sa.x = f64_ptr(ctx, B200SPH_X); sa.y = f64_ptr(ctx, B200SPH_Y); sa.z = f64_ptr(ctx, B200SPH_Z);
+    sa.u = f64_ptr(ctx, B200SPH_U); sa.v = f64_ptr(ctx, B200SPH_V); sa.w = f64_ptr(ctx, B200SPH_W);
+    sa.uadv = f64_ptr(ctx, B200SPH_UADV); sa.vadv = f64_ptr(ctx, B200SPH_VADV); sa.wadv = f64_ptr(ctx, B200SPH_WADV);
+    sa.au = f32_ptr(ctx, B200SPH_AU); sa.av = f32_ptr(ctx, B200SPH_AV); sa.aw = f32_ptr(ctx, B200SPH_AW);
+    sa.ptype = ctx->ptype;
+    sa.pool_end = ctx->pool_end;
+    sa.mask = arr < 0 ? ~0u : 1u << arr;
+    sa.dt = dt;
+    sa.tc = devdt ? ctx->tc : nullptr;
+    if (ctx->pool_end > 0) {
+        k_stage_iisph<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
+        LAUNCH_CHECK();
+    }
+    particles_moved(ctx);
+    return 0;
+}
+int b200sph_stage_iisph(b200sph_ctx *ctx, int arr, int which, double dt) { return stage_iisph_impl(ctx, arr, which, dt, false); }
+int b200sph_stage_iisph_dev(b200sph_ctx *ctx, int arr, int which) { return stage_iisph_impl(ctx, arr, which, 0.0, true); }
 
 // the fused stage kernel applies when one launch steps every array (arr == -1) and the
 // neighbour lists of the current build can be reused: then the records of the next

@@ -96,10 +96,13 @@ __global__ void k_shift_vmax(const double *__restrict__ u, const double *__restr
     if ((threadIdx.x & 31) == 0 && vm > 0.0) atomicMax(out, __double_as_longlong(vm));
 }
 
+// (these three helpers take any argument block with the ShiftArgs geometry fields: the IISPH
+// passes share them)
 // x_ij = x_i - (x_j + image) of list entry e in fp64 and r^2 as the reference forms them.  The
 // entry's cell offset d puts the source in the apparent cell c_i + d; where that differs from
 // its own cell of the build (a periodic wrap), the image is the source shifted by the box.
-__device__ __forceinline__ double shift_dist(const ShiftArgs &a, const uint32_t e, const ShiftRec &Pi, const ShiftRec &Pj,
+template <class A>
+__device__ __forceinline__ double shift_dist(const A &a, const uint32_t e, const ShiftRec &Pi, const ShiftRec &Pj,
                                              const uint32_t ci[3], const uint32_t keyj, double xij[3])
 {
     uint32_t cj[3];
@@ -116,15 +119,16 @@ __device__ __forceinline__ double shift_dist(const ShiftArgs &a, const uint32_t 
 }
 
 // linked_list_nnps.pyx:188 in fp64: r^2 < (k h_i)^2 or r^2 < (k h_j)^2
-__device__ __forceinline__ bool shift_accept(const ShiftArgs &a, const double r2, const double hi, const double hj)
+template <class A>
+__device__ __forceinline__ bool shift_accept(const A &a, const double r2, const double hi, const double hj)
 {
     const double ki = shift_mul(a.kr, hi), kj = shift_mul(a.kr, hj);
     return r2 < shift_mul(ki, ki) || r2 < shift_mul(kj, kj);
 }
 
 // W(r, h) and grad W(x, r, h) (kernels.py) with the kernel polynomial in fp32
-template <int K, int DIM>
-__device__ __forceinline__ void shift_kernel(const ShiftArgs &a, const double xij[3], const double rij, const double hij,
+template <int K, int DIM, class A>
+__device__ __forceinline__ void shift_kernel(const A &a, const double xij[3], const double rij, const double hij,
                                              double &wij, double dwij[3])
 {
     const double h1 = 1.0 / hij;

@@ -37,6 +37,7 @@ _SUPPORTED_STEPPERS = {
     'EDACStep': ('b200sph_stage_edac', 'b200sph_stage_edac_dev'),    # wc/edac.py:82-133
     'SolidMechStep': ('b200sph_stage_solid', 'b200sph_stage_solid_dev'),   # integrator_step.py:173-252
     'WCSPHTVDRK3Step': ('b200sph_stage_rk3', 'b200sph_stage_rk3_dev'),
+    'IISPHStep': ('b200sph_stage_iisph', 'b200sph_stage_iisph_dev'),   # iisph.py:22-34
 }
 
 
@@ -140,17 +141,23 @@ class B200Integrator(object):
             if pm:
                 pm.update(deferred=True)
             self.nnps.update(deferred=True)
-        self.acceleration_evals[index].compute(self.t, self.dt)
+        ae = self.acceleration_evals[index]
+        ae.device_dt = self.device_dt
+        ae.compute(self.t, self.dt)
         if update_nnps:
             redo = pm.confirm() if pm else False
             redo = self.nnps.confirm() or redo
             if redo:
+                # (an IISPH evaluation starts the repeat from the pressure the first attempt
+                # started from: the library restores it)
                 self.nnps.update()
-                self.acceleration_evals[index].compute(self.t, self.dt)
+                ae.compute(self.t, self.dt)
 
     def initial_acceleration(self, t, dt):
         # integrator.py:289-297: evaluate once WITHOUT refreshing the NNPS
-        self.acceleration_evals[0].compute(t, dt)
+        ae = self.acceleration_evals[0]
+        ae.device_dt = self.device_dt
+        ae.compute(t, dt)
 
     def step(self, time, dt):
         # integrator_cython.mako:76-82
@@ -179,6 +186,10 @@ class B200Integrator(object):
 
 
 class EulerIntegrator(B200Integrator):
+    """integrator.py:312-327.  IISPHStep (iisph.py:22-34) is the only stepper with a device
+    stage 1 under it: with any other, stage1 raises."""
+    steppers_supported = B200Integrator.steppers_supported + ('IISPHStep',)
+
     def one_timestep(self, t, dt):   # integrator.py:322-327
         self.compute_accelerations()
         self.stage1()
@@ -186,8 +197,10 @@ class EulerIntegrator(B200Integrator):
         self.do_post_stage(dt, 1)
 
     def stage1(self):
-        raise NotImplementedError(
-            'EulerStep has no device kernel on the B200 backend')
+        if any(s.__class__.__name__ != 'IISPHStep' for s in self.steppers.values()):
+            raise NotImplementedError(
+                'EulerStep has no device kernel on the B200 backend')
+        self._stage(1, self.dt)
 
 
 class PECIntegrator(B200Integrator):

@@ -12,6 +12,7 @@ recognises each equation by *class name* and maps every Group onto
     ('dfilter', mode, array_mask, real_only)              density re-initialisation
     ('shift', kind, array_mask, coef, hdx, tensile, R, n)  particle shifting (dt: compute's)
     ('correct_vel', array_mask)                            CorrectVelocities after a shift
+    ('iisph', IisphProgram, fluid_indices)                 IISPHScheme's Groups, as a whole
 
 Anything the CUDA library has no kernel for raises NotImplementedError here,
 i.e. at setup time, never silently at run time.
@@ -446,9 +447,88 @@ def build_program(groups, array_names, dim, particle_arrays=None, kernel=None, g
     arrays = dict((pa.name, pa) for pa in (particle_arrays or []))
     arrays['__codegen__'] = (kernel, int(dim), generic)
     ops = []
-    for g in group_equations(groups):
-        ops.extend(_mega_group(g, index, arrays, particle_arrays))
+    groups = group_equations(groups)
+    i = 0
+    while i < len(groups):
+        found = _match_iisph(groups, i, index)
+        if found:
+            ops.append(found[0])
+            i += found[1]
+            continue
+        ops.extend(_mega_group(groups[i], index, arrays, particle_arrays))
+        i += 1
     return _merge_solid(_merge_tvf(ops))
+
+
+# ---- IISPHScheme (pysph/sph/iisph.py:511-643) ---------------------------------------------------
+_IISPH_PARAMS = ('rho0', 'nu', 'gx', 'gy', 'gz', 'omega', 'tolerance')
+
+
+def _iisph_signature(g, top=True):
+    """What must agree between a Group and the one IISPHScheme.get_equations emits: the
+    flags, the sub-groups, and per equation its class (SummationDensity: of an iisph module),
+    destination, sources and parameters.  An iterated Group's iteration limits are taken as
+    given, not compared."""
+    flags = (bool(getattr(g, 'real', True)), bool(getattr(g, 'iterate', False)) if top else False,
+             bool(getattr(g, 'update_nnps', False)), getattr(g, 'pre', None) is None,
+             getattr(g, 'post', None) is None, getattr(g, 'condition', None) is None,
+             getattr(g, 'start_idx', 0) in (0, None), getattr(g, 'stop_idx', None) is None)
+    if getattr(g, 'has_subgroups', False):
+        return flags + (tuple(_iisph_signature(sg, False) for sg in g.equations),)
+    eqs = []
+    for eq in g.equations:
+        name = _eq_name(eq)
+        if name == 'SummationDensity' and 'iisph' not in eq.__class__.__module__:
+            name = 'other SummationDensity'
+        eqs.append((name, eq.dest, tuple(eq.sources or ())) +
+                   tuple((k, float(getattr(eq, k))) for k in _IISPH_PARAMS if hasattr(eq, k)))
+    return flags + (tuple(eqs),)
+
+
+def _match_iisph(groups, i, index):
+    """(('iisph', IisphProgram, fluid indices), number of Groups) when groups[i:] begins with
+    the Groups of an IISPHScheme -- the same Groups, in the same order, that its get_equations
+    emits for the fluids, solids and parameters they name -- else None.  Groups that do not
+    form the scheme are translated one by one as before (the generic fallback included)."""
+    from .iisph import IISPHScheme
+    for n in (7, 5):
+        gs = groups[i:i + n]
+        if len(gs) != n:
+            continue
+        try:
+            k = 2 if n == 7 else 0
+            dens = gs[1 if n == 7 else 0].equations
+            fluids = [eq.dest for eq in dens]
+            solids = list(gs[2].equations[0].sources) if n == 7 else []
+            adv = gs[k + 1].equations[0]
+            iters = gs[k + 3]
+            ps = [eq for sg in iters.equations for eq in sg.equations
+                  if _eq_name(eq) == 'PressureSolve'][0]
+            nu = max([float(eq.nu) for eq in gs[k + 1].equations if hasattr(eq, 'nu')] or [0.0])
+            has_ghosts = len(iters.equations) == 4
+            want = IISPHScheme(fluids, solids, 0, float(ps.rho0), nu=nu, gx=float(adv.gx),
+                               gy=float(adv.gy), gz=float(adv.gz), omega=float(ps.omega),
+                               tolerance=float(ps.tolerance),
+                               has_ghosts=has_ghosts).get_equations()
+        except (AttributeError, IndexError, TypeError, ValueError):
+            continue
+        if len(want) != n or any(_iisph_signature(a) != _iisph_signature(b)
+                                 for a, b in zip(gs, want)):
+            continue
+        if any(a not in index for a in fluids + solids):
+            raise ValueError('IISPHScheme: unknown particle array among %r' % (fluids + solids))
+        prog = _lib.IisphProgram()
+        for f in fluids:
+            prog.fluid_mask |= 1 << index[f]
+        for sd in solids:
+            prog.solid_mask |= 1 << index[sd]
+        prog.rho0, prog.nu = float(ps.rho0), nu
+        prog.gx, prog.gy, prog.gz = float(adv.gx), float(adv.gy), float(adv.gz)
+        prog.omega, prog.tolerance = float(ps.omega), float(ps.tolerance)
+        prog.min_iterations = int(getattr(iters, 'min_iterations', 0))
+        prog.max_iterations = int(getattr(iters, 'max_iterations', 1))
+        return ('iisph', prog, tuple(sorted(index[f] for f in fluids))), n
+    return None
 
 
 def _wrap(g, body, top):

@@ -168,6 +168,9 @@ class B200Solver(object):
                                                    getattr(dom, 'is_mirror', False)):
             raise NotImplementedError(
                 'B200 backend: periodic / mirror domains with the slab decomposition')
+        if pm is not None and any('uadv' in pa.properties for pa in self.particles):
+            # (b200sph_iisph_pass refuses it too; IISPH arrays keep p where EDAC keeps its own)
+            raise NotImplementedError('B200 backend: IISPHScheme with the slab decomposition')
         if pm is not None:
             from ._lib import EDAC_PROP_IDS
             # (the per-array tables are copies: compare what an EDAC table maps p to)
