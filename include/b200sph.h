@@ -83,6 +83,12 @@ enum {
     B200SPH_DII0 = 144, B200SPH_DII1, B200SPH_DII2, B200SPH_AII,
     B200SPH_DIJPJ0 = 148, B200SPH_DIJPJ1, B200SPH_DIJPJ2, B200SPH_PITER,
     B200SPH_COMPRESSION = 152, B200SPH_IISPH_V = 153,
+    /* generalised transport-velocity extension (get_particle_array_gtvf, pysph/sph/wc/gtvf.py:
+     * 32-49), fp64, device memory allocated as one group on first use: CorrectDensity's rhodiv
+     * and MomentumEquationPressureGradient's p0.  A GTVF fluid keeps uhat .. what and
+     * auhat .. awhat in the transport-velocity slots, rho0 in B200SPH_RHO0 and p in the fp64
+     * B200SPH_PF; a GTVF wall uses the EDAC wall layout (b200sph_tvf_program). */
+    B200SPH_RHODIV = 131, B200SPH_GTVF_P0 = 132,
     /* 32-bit integer props */
     B200SPH_GID = 64, B200SPH_TAG = 65, B200SPH_PID = 66,
     /* fp64 properties the pool does not know, created on first use for the generic-equation
@@ -171,6 +177,24 @@ typedef struct {
     int32_t dt_device;     /* ... or, != 0, dt from the device time-control block       */
     int32_t reserved;
 } b200sph_iisph_program;
+
+/* The two evaluations of GTVFScheme.get_equations (pysph/sph/wc/gtvf.py:586-662), a
+ * MultiStageEquations.  Evaluation 0: SetWallVelocity of every wall over the fluids, then
+ * ContinuityEquationGTVF over the fluids and ContinuitySolid over the walls.  Evaluation 1:
+ * CorrectDensity over every array and StateEquation(p0 = pref, rho0, b = 1); VolumeSummation over
+ * every array and the transport-velocity SolidWallPressureBC(rho0, p0 = pref, b = 1, g) of every
+ * wall over the fluids; MomentumEquationPressureGradient(pref, g) over every array,
+ * MomentumEquationArtificialViscosity(c0, alpha) (alpha > 0), MomentumEquationViscosity(nu)
+ * (nu > 0) and MomentumEquationArtificialStress over the fluids. */
+typedef struct {
+    uint32_t fluid_mask;   /* bit a: array a is a fluid (one fluid array)               */
+    uint32_t solid_mask;   /* bit a: array a is a wall (0: none)                        */
+    double rho0;           /* the scheme's reference density                            */
+    double pref;           /* reference pressure (StateEquation, SolidWallPressureBC, p0) */
+    double c0, alpha;      /* MomentumEquationArtificialViscosity (alpha 0: absent)     */
+    double nu;             /* MomentumEquationViscosity (0: absent; refused with walls) */
+    double gx, gy, gz;
+} b200sph_gtvf_program;
 
 /* The two Groups of ElasticSolidsScheme.get_equations (solid_mech/basic.py:604-651) for
  * elastic solids (destinations and sources) and rigid `solids` (sources only).  Group 1: IsothermalEOS (:93-101), VelocityGradient2D/3D
@@ -472,6 +496,18 @@ int b200sph_iisph_stats(b200sph_ctx *ctx, int *iterations, double compression[B2
 /* IISPHStep.stage1 (iisph.py:22-34): u = uadv + dt au, x += dt u (which must be 1) */
 int b200sph_stage_iisph(b200sph_ctx *ctx, int arr, int which, double dt);
 int b200sph_stage_iisph_dev(b200sph_ctx *ctx, int arr, int which);
+
+/* One GTVF evaluation (see b200sph_gtvf_program), evaluation 0 or 1, on the persistent neighbour
+ * lists.  Evaluation 0 runs on the lists as they are (the positions have not moved since the
+ * last update); evaluation 1 may run on a deferred drift check, and when it repeats after that
+ * check failed (b200sph_nnps_confirm) it starts from the density stage 2 produced, which the
+ * first attempt kept in rho0.  Refused: several fluid arrays, nu > 0 with walls, the slab
+ * decomposition, mirror domains, ghost particles, 1-D. */
+int b200sph_gtvf_pass(b200sph_ctx *ctx, const b200sph_gtvf_program *prog, int evaluation);
+/* GTVFStep (gtvf.py:70-98), which = 1, 2 or 3: u += dt/2 au, uhat = u + dt/2 auhat | rho += dt
+ * arho, x += dt uhat | u += dt/2 au */
+int b200sph_stage_gtvf(b200sph_ctx *ctx, int arr, int which, double dt);
+int b200sph_stage_gtvf_dev(b200sph_ctx *ctx, int arr, int which);
 
 /* The elastic-dynamics evaluation (see b200sph_solid_program); same neighbour lists as
  * pair_pass. */

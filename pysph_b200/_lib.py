@@ -45,6 +45,10 @@ IISPH_PROP_IDS = dict(PROP_IDS, p=30, p0=31, V=153)
 IISPH_PROP_IDS.update((n, 140 + i) for i, n in enumerate(
     ('uadv', 'vadv', 'wadv', 'rho_adv', 'dii0', 'dii1', 'dii2', 'aii', 'dijpj0', 'dijpj1',
      'dijpj2', 'piter', 'compression')))
+# generalised transport-velocity extension (B200SPH_RHODIV, B200SPH_GTVF_P0); GTVF fluids (they own
+# 'rhodiv' and are no wall) keep p in the fp64 B200SPH_PF and rho0 in B200SPH_RHO0; GTVF walls use
+# EDAC_WALL_PROP_IDS
+GTVF_PROP_IDS = dict(PROP_IDS, p=30, rhodiv=131, p0=132)
 INT_PROP_IDS = {'gid': 64, 'tag': 65, 'pid': 66}
 USER_PROP0, MAX_USER_PROPS = 110, 16     # B200SPH_USER0, B200SPH_MAX_USER
 F64_DEVICE_PROPS = ('x', 'y', 'z', 'u', 'v', 'w', 'rho', 'h', 'm',
@@ -112,6 +116,13 @@ class IisphProgram(C.Structure):
                 ('omega', C.c_double), ('tolerance', C.c_double),
                 ('min_iterations', C.c_int32), ('max_iterations', C.c_int32),
                 ('dt', C.c_double), ('dt_device', C.c_int32), ('reserved', C.c_int32)]
+
+
+class GtvfProgram(C.Structure):
+    _fields_ = [('fluid_mask', C.c_uint32), ('solid_mask', C.c_uint32),
+                ('rho0', C.c_double), ('pref', C.c_double),
+                ('c0', C.c_double), ('alpha', C.c_double), ('nu', C.c_double),
+                ('gx', C.c_double), ('gy', C.c_double), ('gz', C.c_double)]
 
 
 class GridInfo(C.Structure):
@@ -199,6 +210,9 @@ SIGNATURES = {
     'b200sph_iisph_stats': (C.c_int, [_ctx_p, C.POINTER(C.c_int), _dp]),
     'b200sph_stage_iisph': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_double]),
     'b200sph_stage_iisph_dev': (C.c_int, [_ctx_p, C.c_int, C.c_int]),
+    'b200sph_gtvf_pass': (C.c_int, [_ctx_p, C.POINTER(GtvfProgram), C.c_int]),
+    'b200sph_stage_gtvf': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_double]),
+    'b200sph_stage_gtvf_dev': (C.c_int, [_ctx_p, C.c_int, C.c_int]),
     'b200sph_stage': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_double]),
     'b200sph_dt_factors': (C.c_int, [_ctx_p, _dp]),
     'b200sph_time_control': (C.c_int, [_ctx_p, C.c_void_p, C.POINTER(C.c_void_p)]),

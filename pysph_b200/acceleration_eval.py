@@ -165,6 +165,8 @@ class B200AccelerationEval(object):
                 prog.dt_device = 1 if self.device_dt else 0
                 ctx.call('b200sph_iisph_pass', C.byref(prog), C.byref(cnt) if self.count_pairs else None)
                 self._pairs += cnt.value if self.count_pairs else 0
+            elif kind == 'gtvf':
+                ctx.call('b200sph_gtvf_pass', C.byref(op[1]), op[2])
             elif kind == 'update_nnps':
                 # mako:139-145: nnps.update_domain(); nnps.update()
                 ctx.call('b200sph_update_domain')

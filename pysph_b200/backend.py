@@ -13,7 +13,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import (PROP_IDS, INT_PROP_IDS, EDAC_PROP_IDS, EDAC_WALL_PROP_IDS,
-                   ELASTIC_PROP_IDS, IISPH_PROP_IDS)
+                   ELASTIC_PROP_IDS, IISPH_PROP_IDS, GTVF_PROP_IDS)
 
 
 def _host_array(pa, name):
@@ -74,12 +74,14 @@ class B200Backend(object):
         self.index = dict((n, i) for i, n in enumerate(self.names))
         # name -> device property id, per array: EDAC arrays evolve p (fp64 PF)
         # (a wall of the EDAC scheme may carry 'ap' too, wc/edac.py:46-47: walls first);
-        # IISPH arrays keep p, the warm start of the pressure solve, in PF too
+        # IISPH arrays keep p, the warm start of the pressure solve, in PF too; so do GTVF fluids
+        # (a GTVF wall carries rhodiv too: walls first)
         self.prop_ids = [dict(EDAC_WALL_PROP_IDS if 'wij' in pa.properties and
                               'ug' in pa.properties else
                               (EDAC_PROP_IDS if 'ap' in pa.properties else
                                (ELASTIC_PROP_IDS if 's00' in pa.properties else
-                                (IISPH_PROP_IDS if 'uadv' in pa.properties else PROP_IDS))))
+                                (IISPH_PROP_IDS if 'uadv' in pa.properties else
+                                 (GTVF_PROP_IDS if 'rhodiv' in pa.properties else PROP_IDS)))))
                          for pa in particle_arrays]
         self.user_props = []      # names of the fp64 properties created for generic equations
         for pa in particle_arrays:

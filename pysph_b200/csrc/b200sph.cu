@@ -22,7 +22,7 @@
 // One translation unit: this file holds the context, the pool and every C-ABI entry
 // point; the kernels are included below by family (pool_kernels, scan, nnps_kernels,
 // sph_kernels, pair_kernel, pair_list, tvf_kernels, solid_kernels, halo_kernels, density_filter,
-// interp_kernels, shift_kernels, iisph_kernels .cuh).
+// interp_kernels, shift_kernels, iisph_kernels, gtvf_kernels .cuh).
 //
 // No CPU fallback: every entry point needs a CUDA device.
 #include "b200sph.h"
@@ -433,6 +433,11 @@ struct b200sph_ctx {
     Buf<double> iisph_pnext, iisph_part;
     Buf<IisphState> iisph_st;
     bool iisph_spec = false, iisph_restore = false;
+    // the generalised transport-velocity formulation (b200sph_gtvf_pass): the position records
+    // [n_sorted].  gtvf_spec: an evaluation 1 ran on a deferred drift check not yet confirmed;
+    // gtvf_restore: that check failed, so the repeat keeps rho0 (the density of stage 2)
+    Buf<ShiftRec> gtvf_P;
+    bool gtvf_spec = false, gtvf_restore = false;
     // Group(start_idx, stop_idx): one-shot destination ranges of the next pair pass
     int64_t dst_lo[B200SPH_MAX_ARRAYS] = {0}, dst_hi[B200SPH_MAX_ARRAYS] = {0};
     bool dst_ranged = false;
@@ -718,6 +723,7 @@ __device__ __forceinline__ void rec32_make(const float4 A, const double u, const
 #include "interp_kernels.cuh"
 #include "shift_kernels.cuh"
 #include "iisph_kernels.cuh"
+#include "gtvf_kernels.cuh"
 
 // --------------------------------------------------------------------------
 // host side
@@ -728,7 +734,7 @@ __device__ __forceinline__ void rec32_make(const float4 A, const double u, const
 // time any IISPH property is named, or one by one when a
 // user property is named.  The only host code that knows the ranges of the id enum.
 enum PropType { PROP_NONE, PROP_F64, PROP_F32, PROP_U32 };
-enum PropGroup { GROUP_POOL, GROUP_ELASTIC, GROUP_IISPH, GROUP_USER };
+enum PropGroup { GROUP_POOL, GROUP_ELASTIC, GROUP_IISPH, GROUP_GTVF, GROUP_USER };
 struct PropKind {
     PropType type;
     PropGroup group;
@@ -744,6 +750,7 @@ static PropKind prop_kind(int p)
     if (p >= B200SPH_S00 && p <= B200SPH_S220) return {PROP_F64, GROUP_ELASTIC};
     if (p >= B200SPH_V00 && p <= B200SPH_AS22) return {PROP_F32, GROUP_ELASTIC};
     if (p >= B200SPH_UADV && p <= B200SPH_IISPH_V) return {PROP_F64, GROUP_IISPH};
+    if (p >= B200SPH_RHODIV && p <= B200SPH_GTVF_P0) return {PROP_F64, GROUP_GTVF};
     if (p >= B200SPH_USER0 && p < B200SPH_USER0 + B200SPH_MAX_USER) return {PROP_F64, GROUP_USER};
     return {PROP_NONE, GROUP_POOL};
 }
@@ -1770,8 +1777,10 @@ static int confirm_pending(b200sph_ctx *ctx, int *redo)
         ctx->n_deferred_failed++;
         *redo = 1;
         ctx->iisph_restore = ctx->iisph_spec;
+        ctx->gtvf_restore = ctx->gtvf_spec;
     }
     ctx->iisph_spec = false;
+    ctx->gtvf_spec = false;
     return 0;
 }
 // entry points that consume the results of an evaluation must not run on an
@@ -3440,6 +3449,153 @@ static int stage_iisph_impl(b200sph_ctx *ctx, int arr, int which, double dt, boo
 }
 int b200sph_stage_iisph(b200sph_ctx *ctx, int arr, int which, double dt) { return stage_iisph_impl(ctx, arr, which, dt, false); }
 int b200sph_stage_iisph_dev(b200sph_ctx *ctx, int arr, int which) { return stage_iisph_impl(ctx, arr, which, 0.0, true); }
+
+// ---- the generalised transport-velocity formulation (gtvf_kernels.cuh) -------------------------
+// A list consumer like the IISPH pass.  Evaluation 0 runs without a neighbour-search update
+// (GTVFIntegrator, gtvf.py:57): the positions are those of the last update, so the lists of that
+// update serve it as they are.  Evaluation 1 may run on a deferred drift check; CorrectDensity
+// moves rho into rho0 before it rewrites rho, so a repeat after a failed check keeps rho0 (the
+// density stage 2 produced) instead of taking the first attempt's rho.
+int b200sph_gtvf_pass(b200sph_ctx *ctx, const b200sph_gtvf_program *prog, int evaluation)
+{
+    CU(cudaSetDevice(ctx->device));
+    int rc = ensure_pool(ctx);
+    if (rc) return rc;
+    const unsigned fm = prog->fluid_mask, sm = prog->solid_mask;
+    if (evaluation != 0 && evaluation != 1) return set_err(ctx, "gtvf_pass: evaluation must be 0 or 1 (got %d)", evaluation);
+    if (fm == 0 || fm >= (1u << ctx->narr) || (fm & (fm - 1)))
+        return set_err(ctx, "gtvf_pass: bad fluid mask 0x%x (one fluid array)", fm);
+    if (sm >= (1u << ctx->narr) || (sm & fm)) return set_err(ctx, "gtvf_pass: bad solid mask 0x%x (fluid 0x%x)", sm, fm);
+    if (prog->nu > 0.0 && sm) return set_err(ctx, "gtvf_pass: nu > 0 with walls (SolidWallNoSlipBC reads a V the fluid does not have)");
+    if (!(prog->pref != 0.0) || !(prog->rho0 != 0.0)) return set_err(ctx, "gtvf_pass: pref and rho0 must be non-zero");
+    if (ctx->dim < 2) return set_err(ctx, "gtvf_pass: GTVF runs in 2-D and 3-D");
+    if (ctx->peer_box || ctx->comm_pending) return set_err(ctx, "gtvf_pass runs on one GPU (no slab decomposition)");
+    if (mirror_any(ctx)) return set_err(ctx, "gtvf_pass: mirror domains are not supported");
+    for (int a = 0; a < ctx->narr; a++)
+        if (ctx->arr[a].n != ctx->arr[a].n_real)
+            return set_err(ctx, "gtvf_pass: array '%s' has ghost particles", ctx->arr[a].name.c_str());
+    if (!ctx->grid_valid) return set_err(ctx, "gtvf_pass: the NNPS is stale (particles were pushed, resized or moved); call nnps_update first");
+    if ((rc = ensure_prop(ctx, B200SPH_RHODIV))) return rc;
+    if ((rc = eos_flush(ctx)) || (rc = ab_positions(ctx))) return rc;
+    if (evaluation == 1) {
+        // CorrectDensity.initialize (gtvf.py:138-141): rho0 = rho -- unless this is the repeat of
+        // an evaluation whose drift check failed, which already did it
+        if (!ctx->gtvf_restore)
+            for (int a = 0; a < ctx->narr; a++)
+                if (((fm >> a) & 1u) && ctx->arr[a].n > 0)
+                    CU(cudaMemcpyAsync(f64_ptr(ctx, B200SPH_RHO0) + ctx->arr[a].off, f64_ptr(ctx, B200SPH_RHO) + ctx->arr[a].off,
+                                       8 * (size_t)ctx->arr[a].n, cudaMemcpyDeviceToDevice, ctx->stream));
+        ctx->gtvf_restore = false;
+        ctx->gtvf_spec = ctx->check_pending;
+    }
+    if (ctx->n_sorted == 0) return 0;
+    unsigned long long want[B200SPH_MAX_ARRAYS] = {0};
+    for (int a = 0; a < ctx->narr; a++) {
+        if ((fm >> a) & 1u)
+            for (int b = 0; b < ctx->narr; b++)
+                if (((fm | sm) >> b) & 1u) want[a] |= 0xFFull << (8 * b);
+        if ((sm >> a) & 1u)
+            for (int b = 0; b < ctx->narr; b++)
+                if (((fm | sm) >> b) & 1u) want[a] |= 0xFFull << (8 * b);
+    }
+    if ((rc = prepare_lists(ctx, want, "gtvf_pass: the neighbour lists cannot index the particles"))) return rc;
+    const size_t n = (size_t)ctx->n_sorted;
+    if ((rc = grow(ctx, ctx->gtvf_P, n, n))) return rc;
+    GtvfArgs ga;
+    memset(&ga, 0, sizeof(ga));
+    ga.P = ctx->gtvf_P;
+    ga.perm = ctx->perm; ga.cnt = ctx->cnt; ga.lst = ctx->lst; ga.skey = ctx->skey; ga.stype = ctx->stype;
+    ga.x = f64_ptr(ctx, B200SPH_X); ga.y = f64_ptr(ctx, B200SPH_Y); ga.z = f64_ptr(ctx, B200SPH_Z);
+    ga.h = f64_ptr(ctx, B200SPH_H); ga.m = f64_ptr(ctx, B200SPH_M);
+    ga.u = f64_ptr(ctx, B200SPH_U); ga.v = f64_ptr(ctx, B200SPH_V); ga.w = f64_ptr(ctx, B200SPH_W);
+    // a fluid's uhat .. what and a wall's ug .. wg share the transport-velocity slots
+    ga.uh = f64_ptr(ctx, B200SPH_UHAT); ga.vh = f64_ptr(ctx, B200SPH_VHAT); ga.wh = f64_ptr(ctx, B200SPH_WHAT);
+    ga.ug = f64_ptr(ctx, B200SPH_UHAT); ga.vg = f64_ptr(ctx, B200SPH_VHAT); ga.wg = f64_ptr(ctx, B200SPH_WHAT);
+    ga.rho = f64_ptr(ctx, B200SPH_RHO); ga.rho0 = f64_ptr(ctx, B200SPH_RHO0);
+    ga.pf = f64_ptr(ctx, B200SPH_PF); ga.rhodiv = f64_ptr(ctx, B200SPH_RHODIV); ga.p0 = f64_ptr(ctx, B200SPH_GTVF_P0);
+    ga.p = f32_ptr(ctx, B200SPH_P); ga.arho = f32_ptr(ctx, B200SPH_ARHO);
+    ga.au = f32_ptr(ctx, B200SPH_AU); ga.av = f32_ptr(ctx, B200SPH_AV); ga.aw = f32_ptr(ctx, B200SPH_AW);
+    // a fluid's auhat .. awhat and a wall's uf .. wf share these slots too
+    ga.auh = f32_ptr(ctx, B200SPH_AUHAT); ga.avh = f32_ptr(ctx, B200SPH_AVHAT); ga.awh = f32_ptr(ctx, B200SPH_AWHAT);
+    ga.uf = f32_ptr(ctx, B200SPH_AUHAT); ga.vf = f32_ptr(ctx, B200SPH_AVHAT); ga.wf = f32_ptr(ctx, B200SPH_AWHAT);
+    ga.vol = f32_ptr(ctx, B200SPH_VOL); ga.wij = f32_ptr(ctx, B200SPH_PAVG);
+    ga.n = ctx->n_sorted; ga.capg = ctx->capg;
+    ga.ncx = ctx->G.nc[0]; ga.ncy = ctx->G.nc[1]; ga.zorder = ctx->G.zorder;
+    for (int d = 0; d < 3; d++) {
+        ga.per[d] = ctx->G.periodic[d];
+        ga.L[d] = ctx->dom_hi[d] - ctx->dom_lo[d];
+    }
+    ga.kr = ctx->radius_scale;
+    ga.kfac = kernel_fac(ctx->kernel, ctx->dim);
+    ga.fluid_mask = fm; ga.solid_mask = sm;
+    ga.rho0c = prog->rho0; ga.pref = prog->pref; ga.c0 = prog->c0; ga.alpha = prog->alpha; ga.nu = prog->nu;
+    ga.gx = prog->gx; ga.gy = prog->gy; ga.gz = prog->gz;
+    PhaseTimer pt(ctx, 2);
+    k_gtvf_pack<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(ga);
+    LAUNCH_CHECK();
+    const unsigned nb = (unsigned)cdiv(ctx->n_sorted, GTVF_NT);
+    const auto pass = [&](const int which) {
+        return with_kernel_dim(ctx, "gtvf_pass", [&](auto kc, auto dc) {
+            constexpr int K = decltype(kc)::value, D = decltype(dc)::value;
+            switch (which) {
+            case GTVF_WALLV: k_gtvf<K, D, GTVF_WALLV><<<nb, GTVF_NT, 0, ctx->stream>>>(ga); break;
+            case GTVF_CONT: k_gtvf<K, D, GTVF_CONT><<<nb, GTVF_NT, 0, ctx->stream>>>(ga); break;
+            case GTVF_RHO: k_gtvf<K, D, GTVF_RHO><<<nb, GTVF_NT, 0, ctx->stream>>>(ga); break;
+            case GTVF_WALLP: k_gtvf<K, D, GTVF_WALLP><<<nb, GTVF_NT, 0, ctx->stream>>>(ga); break;
+            default: k_gtvf<K, D, GTVF_MOM><<<nb, GTVF_NT, 0, ctx->stream>>>(ga); break;
+            }
+            LAUNCH_CHECK();
+            return 0;
+        });
+    };
+    if (evaluation == 0) {
+        if (sm && (rc = pass(GTVF_WALLV))) return rc;
+        if ((rc = pass(GTVF_CONT))) return rc;
+    } else {
+        if ((rc = pass(GTVF_RHO))) return rc;
+        if (sm && (rc = pass(GTVF_WALLP))) return rc;
+        if ((rc = pass(GTVF_MOM))) return rc;
+    }
+    ctx->stats.pair_launches++;
+    pt.stop();
+    // rho, p and the accelerations changed: the next evaluation packs its records from the pool
+    state_changed(ctx);
+    ctx->spec_records = false;
+    return 0;
+}
+
+static int stage_gtvf_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devdt)
+{
+    int rc = stage_begin(ctx, "stage_gtvf", arr, which, devdt, 3);
+    if (rc) return rc;
+    if (which < 1) return set_err(ctx, "stage_gtvf: GTVFStep has stages 1, 2 and 3 (got %d)", which);
+    PhaseTimer pt(ctx, 2);
+    StageGtvfArgs sa;
+    sa.x = f64_ptr(ctx, B200SPH_X); sa.y = f64_ptr(ctx, B200SPH_Y); sa.z = f64_ptr(ctx, B200SPH_Z);
+    sa.u = f64_ptr(ctx, B200SPH_U); sa.v = f64_ptr(ctx, B200SPH_V); sa.w = f64_ptr(ctx, B200SPH_W);
+    sa.uh = f64_ptr(ctx, B200SPH_UHAT); sa.vh = f64_ptr(ctx, B200SPH_VHAT); sa.wh = f64_ptr(ctx, B200SPH_WHAT);
+    sa.rho = f64_ptr(ctx, B200SPH_RHO);
+    sa.au = f32_ptr(ctx, B200SPH_AU); sa.av = f32_ptr(ctx, B200SPH_AV); sa.aw = f32_ptr(ctx, B200SPH_AW);
+    sa.auh = f32_ptr(ctx, B200SPH_AUHAT); sa.avh = f32_ptr(ctx, B200SPH_AVHAT); sa.awh = f32_ptr(ctx, B200SPH_AWHAT);
+    sa.arho = f32_ptr(ctx, B200SPH_ARHO);
+    sa.ptype = ctx->ptype;
+    sa.pool_end = ctx->pool_end;
+    sa.mask = arr < 0 ? ~0u : 1u << arr;
+    sa.which = which;
+    sa.dt = dt;
+    sa.tc = devdt ? ctx->tc : nullptr;
+    if (ctx->pool_end > 0) {
+        k_stage_gtvf<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
+        LAUNCH_CHECK();
+    }
+    // stages 1 and 3 change velocities only: the lists stay valid for evaluation 0, which runs
+    // without a neighbour-search update
+    if (which == 2) particles_moved(ctx);
+    else state_changed(ctx);
+    return 0;
+}
+int b200sph_stage_gtvf(b200sph_ctx *ctx, int arr, int which, double dt) { return stage_gtvf_impl(ctx, arr, which, dt, false); }
+int b200sph_stage_gtvf_dev(b200sph_ctx *ctx, int arr, int which) { return stage_gtvf_impl(ctx, arr, which, 0.0, true); }
 
 // the fused stage kernel applies when one launch steps every array (arr == -1) and the
 // neighbour lists of the current build can be reused: then the records of the next

@@ -58,6 +58,16 @@ class Group(object):
         self.equations = list(equations)
 
 
+class MultiStageEquations(object):
+    """pysph/sph/equation.py:966-995: one list of Groups per evaluation of a multi-stage
+    integrator (GTVFIntegrator evaluates twice per step).  B200Solver builds one
+    B200AccelerationEval per list, as make_acceleration_evals does (acceleration_eval.py:76-90)."""
+
+    def __init__(self, groups):
+        assert type(groups) in (list, tuple)
+        self.groups = groups
+
+
 class SummationDensity(Equation):
     """rho_a = sum_b m_b W_ab   (pysph/sph/basic_equations.py:19-29)"""
 

@@ -38,6 +38,7 @@ _SUPPORTED_STEPPERS = {
     'SolidMechStep': ('b200sph_stage_solid', 'b200sph_stage_solid_dev'),   # integrator_step.py:173-252
     'WCSPHTVDRK3Step': ('b200sph_stage_rk3', 'b200sph_stage_rk3_dev'),
     'IISPHStep': ('b200sph_stage_iisph', 'b200sph_stage_iisph_dev'),   # iisph.py:22-34
+    'GTVFStep': ('b200sph_stage_gtvf', 'b200sph_stage_gtvf_dev'),      # wc/gtvf.py:70-98
 }
 
 

@@ -13,10 +13,13 @@ recognises each equation by *class name* and maps every Group onto
     ('shift', kind, array_mask, coef, hdx, tensile, R, n)  particle shifting (dt: compute's)
     ('correct_vel', array_mask)                            CorrectVelocities after a shift
     ('iisph', IisphProgram, fluid_indices)                 IISPHScheme's Groups, as a whole
+    ('gtvf', GtvfProgram, evaluation)                      one evaluation of GTVFScheme, as a whole
 
 Anything the CUDA library has no kernel for raises NotImplementedError here,
 i.e. at setup time, never silently at run time.
 """
+import numpy as np
+
 from . import _lib
 
 PAIR_EQUATIONS = {
@@ -450,7 +453,7 @@ def build_program(groups, array_names, dim, particle_arrays=None, kernel=None, g
     groups = group_equations(groups)
     i = 0
     while i < len(groups):
-        found = _match_iisph(groups, i, index)
+        found = _match_iisph(groups, i, index) or _match_gtvf(groups, i, index, arrays)
         if found:
             ops.append(found[0])
             i += found[1]
@@ -528,6 +531,90 @@ def _match_iisph(groups, i, index):
         prog.min_iterations = int(getattr(iters, 'min_iterations', 0))
         prog.max_iterations = int(getattr(iters, 'max_iterations', 1))
         return ('iisph', prog, tuple(sorted(index[f] for f in fluids))), n
+    return None
+
+
+# ---- GTVFScheme (pysph/sph/wc/gtvf.py:586-662) -----------------------------------------------
+_GTVF_PARAMS = ('rho0', 'p0', 'b', 'pref', 'gx', 'gy', 'gz', 'c0', 'alpha', 'nu', 'dim')
+
+
+def _gtvf_signature(g):
+    """What must agree between a Group and the one GTVFScheme.get_equations emits: the flags and,
+    per equation, its class and the module it comes from (gtvf or transport_velocity: the EDAC
+    scheme has equations of the same names), destination, sources and parameters."""
+    flags = (bool(getattr(g, 'real', True)), bool(getattr(g, 'iterate', False)),
+             bool(getattr(g, 'update_nnps', False)), getattr(g, 'pre', None) is None,
+             getattr(g, 'post', None) is None, getattr(g, 'condition', None) is None,
+             getattr(g, 'start_idx', 0) in (0, None), getattr(g, 'stop_idx', None) is None,
+             bool(getattr(g, 'has_subgroups', False)))
+    if flags[-1]:
+        return flags              # (the scheme's Groups have no sub-groups)
+    eqs = []
+    for eq in g.equations:
+        mod = eq.__class__.__module__
+        eqs.append((_eq_name(eq), 'gtvf' in mod, 'transport_velocity' in mod, eq.dest,
+                    tuple(eq.sources or ())) +
+                   tuple((k, float(getattr(eq, k))) for k in _GTVF_PARAMS if hasattr(eq, k)))
+    return flags + (tuple(eqs),)
+
+
+def _match_gtvf(groups, i, index, arrays):
+    """(('gtvf', GtvfProgram, evaluation), number of Groups) when groups[i:] is one of the two
+    evaluations GTVFScheme.get_equations emits -- the same Groups, in the same order, for the
+    fluids, walls and parameters they name -- else None.  Several fluid arrays and nu > 0 with
+    walls are refused here."""
+    from .gtvf import GTVFScheme
+    for evaluation, n in ((1, 4), (1, 3), (0, 2), (0, 1)):
+        gs = groups[i:i + n]
+        if len(gs) != n:
+            continue
+        try:
+            if evaluation == 0:
+                cont = gs[-1].equations
+                fluids = [eq.dest for eq in cont if _eq_name(eq) == 'ContinuityEquationGTVF']
+                solids = list(next((eq.sources for eq in cont if _eq_name(eq) == 'ContinuitySolid'), []))
+                kw = dict(dim=2, rho0=1.0, c0=0.0, nu=0.0, h0=None, pref=1.0)
+            else:
+                fluids = [eq.dest for eq in gs[0].equations]
+                solids = [s_ for s_ in gs[0].equations[0].sources if s_ not in fluids]
+                eos = gs[1].equations[0]
+                mom = gs[-1].equations
+                pg = mom[0]
+                av = [eq for eq in mom if _eq_name(eq) == 'MomentumEquationArtificialViscosity']
+                visc = [eq for eq in mom if _eq_name(eq) == 'MomentumEquationViscosity']
+                ast = [eq for eq in mom if _eq_name(eq) == 'MomentumEquationArtificialStress']
+                kw = dict(dim=int(ast[0].dim), rho0=float(eos.rho0), pref=float(pg.pref),
+                          c0=float(av[0].c0) if av else 0.0, alpha=float(av[0].alpha) if av else 0.0,
+                          nu=float(visc[0].nu) if visc else 0.0, h0=None,
+                          gx=float(pg.gx), gy=float(pg.gy), gz=float(pg.gz))
+            want = GTVFScheme(fluids, solids, **kw).get_equations().groups[evaluation]
+            if len(want) != n or any(_gtvf_signature(a) != _gtvf_signature(b) for a, b in zip(gs, want)):
+                continue
+        except (AttributeError, IndexError, TypeError, ValueError, StopIteration):
+            continue
+        if any(a not in index for a in fluids + solids):
+            raise ValueError('GTVFScheme: unknown particle array among %r' % (fluids + solids))
+        if len(fluids) != 1:
+            raise NotImplementedError(
+                'B200 backend: GTVFScheme with %d fluid arrays (the reference runs CorrectDensity '
+                'destination by destination, so a fluid reads a later fluid\'s stale rho0); one '
+                'fluid array is supported' % len(fluids))
+        if evaluation == 1 and kw['nu'] > 0.0 and solids:
+            raise NotImplementedError(
+                'B200 backend: GTVFScheme with nu > 0 and walls (SolidWallNoSlipBC reads the '
+                'fluid\'s V, which GTVF fluid arrays do not have)')
+        for f in fluids:
+            pa = arrays.get(f)
+            if pa is not None and 'asigma' in pa.properties and np.any(pa.properties['asigma'] != 0.0):
+                raise NotImplementedError(
+                    'B200 backend: GTVF fluid %r has a non-zero asigma (sigma and asigma stay on '
+                    'the host; GTVFScheme writes neither)' % f)
+        prog = _lib.GtvfProgram()
+        prog.fluid_mask = sum(1 << index[f] for f in fluids)
+        prog.solid_mask = sum(1 << index[s_] for s_ in solids)
+        for k in ('rho0', 'pref', 'c0', 'alpha', 'nu', 'gx', 'gy', 'gz'):
+            setattr(prog, k, float(kw.get(k, 0.0)))
+        return ('gtvf', prog, evaluation), n
     return None
 
 

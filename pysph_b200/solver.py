@@ -11,6 +11,7 @@ import numpy as np
 
 from .acceleration_eval import B200AccelerationEval
 from .backend import B200Backend
+from .equations import MultiStageEquations
 from .nnps import B200NNPS
 
 EPSILON = np.finfo(float).eps * 2        # solver.py:18
@@ -63,13 +64,17 @@ class B200Solver(object):
         self.backend = backend or B200Backend(
             self.particles, device=device, capacity_factor=capacity_factor,
             extra_capacity=extra_capacity)
-        # Solver.setup, solver.py:186-229
-        self.a_eval = B200AccelerationEval(self.particles, equations, kernel,
-                                           backend=self.backend)
+        # Solver.setup, solver.py:186-229; a MultiStageEquations gives one evaluator per stage,
+        # sharing the backend and the NNPS (make_acceleration_evals, acceleration_eval.py:76-90)
+        stages = equations.groups if isinstance(equations, MultiStageEquations) else [equations]
+        self.a_evals = [B200AccelerationEval(self.particles, groups, kernel, backend=self.backend)
+                        for groups in stages]
+        self.a_eval = self.a_evals[0]
         self.nnps = B200NNPS(kernel.dim, self.particles, backend=self.backend,
                              kernel=kernel, domain=domain)
-        self.a_eval.set_nnps(self.nnps)
-        integrator.set_acceleration_evals([self.a_eval])
+        for ae in self.a_evals:
+            ae.set_nnps(self.nnps)
+        integrator.set_acceleration_evals(self.a_evals)
         integrator.set_nnps(self.nnps)
         integrator.set_fixed_h(fixed_h)
         self._initialised = False
@@ -168,6 +173,8 @@ class B200Solver(object):
                                                    getattr(dom, 'is_mirror', False)):
             raise NotImplementedError(
                 'B200 backend: periodic / mirror domains with the slab decomposition')
+        if pm is not None and any('rhodiv' in pa.properties for pa in self.particles):
+            raise NotImplementedError('B200 backend: GTVFScheme with the slab decomposition')
         if pm is not None and any('uadv' in pa.properties for pa in self.particles):
             # (b200sph_iisph_pass refuses it too; IISPH arrays keep p where EDAC keeps its own)
             raise NotImplementedError('B200 backend: IISPHScheme with the slab decomposition')

@@ -42,3 +42,36 @@ class SolidWallNoSlipBC(Equation):
     def __init__(self, dest, sources, nu):
         self.nu = nu
         super(SolidWallNoSlipBC, self).__init__(dest, sources)
+
+
+class SetWallVelocity(Equation):
+    """transport_velocity.py:84-134: uf = the fluid velocity extrapolated to the wall, ug = 2 u - uf
+    (GTVFScheme's; the EDAC scheme has its own, wc/edac.py:186-230)"""
+
+
+class ContinuitySolid(Equation):
+    """transport_velocity.py:157-173: the continuity equation over a wall's dummy velocity ug"""
+
+
+class StateEquation(Equation):
+    """transport_velocity.py:176-216: p = p0 (rho / rho0 - b)"""
+
+    def __init__(self, dest, sources, p0, rho0, b=1.0):
+        self.b = b
+        self.p0 = p0
+        self.rho0 = rho0
+        super(StateEquation, self).__init__(dest, sources)
+
+
+class SolidWallPressureBC(Equation):
+    """transport_velocity.py:641-736: the fluid pressure extrapolated to a wall particle, and the
+    wall's density from it, rho = rho0 (p / p0 + b) (NOT wc/edac.py's: recognised by its module)"""
+
+    def __init__(self, dest, sources, rho0, p0, b=1.0, gx=0.0, gy=0.0, gz=0.0):
+        self.rho0 = rho0
+        self.p0 = p0
+        self.b = b
+        self.gx = gx
+        self.gy = gy
+        self.gz = gz
+        super(SolidWallPressureBC, self).__init__(dest, sources)
