@@ -89,6 +89,16 @@ enum {
      * auhat .. awhat in the transport-velocity slots, rho0 in B200SPH_RHO0 and p in the fp64
      * B200SPH_PF; a GTVF wall uses the EDAC wall layout (b200sph_tvf_program). */
     B200SPH_RHODIV = 131, B200SPH_GTVF_P0 = 132,
+    /* conservative reproducing-kernel SPH extension (get_particle_array_crksph, pysph/sph/wc/
+     * crksph.py:847-863), fp64, device memory allocated as one group on first use: ids 160 .. 191.
+     * A strided property takes one id per component: bi[a] at B200SPH_CRK_BI0 + a, gradai[g] at
+     * B200SPH_CRK_GRADAI0 + g, gradbi[g][a] at B200SPH_CRK_GRADBI00 + 3 g + a and gradv[a][b] at
+     * B200SPH_CRK_GRADV00 + 3 a + b.  A CRKSPH fluid keeps p in the fp64 B200SPH_PF and u0 .. w0
+     * in the pool's B200SPH_U0 .. B200SPH_W0. */
+    B200SPH_CRK_E = 160, B200SPH_CRK_AE, B200SPH_CRK_CS, B200SPH_CRK_V, B200SPH_CRK_AI,
+    B200SPH_CRK_AU = 165, B200SPH_CRK_AV, B200SPH_CRK_AW,
+    B200SPH_CRK_BI0 = 168, B200SPH_CRK_GRADAI0 = 171, B200SPH_CRK_GRADBI00 = 174,
+    B200SPH_CRK_GRADV00 = 183, B200SPH_CRK_LAST = 191,
     /* 32-bit integer props */
     B200SPH_GID = 64, B200SPH_TAG = 65, B200SPH_PID = 66,
     /* fp64 properties the pool does not know, created on first use for the generic-equation
@@ -195,6 +205,23 @@ typedef struct {
     double nu;             /* MomentumEquationViscosity (0: absent; refused with walls) */
     double gx, gy, gz;
 } b200sph_gtvf_program;
+
+/* The two evaluations of CRKSPHScheme.get_equations (pysph/sph/wc/crksph.py:978-1127), a
+ * MultiStageEquations over one fluid array (sources: the fluid itself).  Evaluation 0:
+ * StateEquation + SpeedOfSound(gamma); NumberDensity; CRKSPHPreStep; CRKSPHSymmetric +
+ * SummationDensityCRKSPH, then StateEquation + SpeedOfSound again; CRKSPHSymmetric +
+ * VelocityGradient; CRKSPHSymmetric + MomentumEquation(g, cl, cq, eta_crit, eta_fold) +
+ * LaminarViscosity(nu, eta) (nu 0: absent).  Evaluation 1: CRKSPHSymmetric +
+ * EnergyEquation(gamma, cl_e, cq_e, eta_crit_e, eta_fold_e). */
+typedef struct {
+    uint32_t fluid_mask;   /* bit a: array a is the fluid (one fluid array)              */
+    uint32_t reserved;
+    double gamma;          /* StateEquation, SpeedOfSound, EnergyEquation                */
+    double gx, gy, gz;     /* MomentumEquation's body force                              */
+    double cl, cq, eta_crit, eta_fold;          /* MomentumEquation                      */
+    double cl_e, cq_e, eta_crit_e, eta_fold_e;  /* EnergyEquation                        */
+    double nu, eta;        /* LaminarViscosity (nu 0: absent)                            */
+} b200sph_crksph_program;
 
 /* The two Groups of ElasticSolidsScheme.get_equations (solid_mech/basic.py:604-651) for
  * elastic solids (destinations and sources) and rigid `solids` (sources only).  Group 1: IsothermalEOS (:93-101), VelocityGradient2D/3D
@@ -508,6 +535,17 @@ int b200sph_gtvf_pass(b200sph_ctx *ctx, const b200sph_gtvf_program *prog, int ev
  * arho, x += dt uhat | u += dt/2 au */
 int b200sph_stage_gtvf(b200sph_ctx *ctx, int arr, int which, double dt);
 int b200sph_stage_gtvf_dev(b200sph_ctx *ctx, int arr, int which);
+
+/* One CRKSPH evaluation (see b200sph_crksph_program), evaluation 0 or 1, on the persistent
+ * neighbour lists.  Both are functions of the positions, velocities, e and the properties an
+ * earlier Group of the same step wrote, so a repeat after a failed deferred drift check gives
+ * what the first attempt would have on fresh lists.  Refused: several fluid arrays, the slab
+ * decomposition, mirror domains, ghost particles, 1-D. */
+int b200sph_crksph_pass(b200sph_ctx *ctx, const b200sph_crksph_program *prog, int evaluation);
+/* CRKSPHStep (crksph.py:884-900), which = 1, 2 or 3: u0 = u | u += dt au | e += dt ae,
+ * x += dt/2 (u + u0) */
+int b200sph_stage_crksph(b200sph_ctx *ctx, int arr, int which, double dt);
+int b200sph_stage_crksph_dev(b200sph_ctx *ctx, int arr, int which);
 
 /* The elastic-dynamics evaluation (see b200sph_solid_program); same neighbour lists as
  * pair_pass. */

@@ -10,13 +10,14 @@ reference (pypr/pysph)      here
 compiled AccelerationEval   :class:`B200AccelerationEval`
 compiled Integrator         :class:`PECIntegrator`, :class:`EPECIntegrator`,
                             :class:`TVDRK3Integrator`, :class:`EulerIntegrator`,
-                            :class:`GTVFIntegrator`
+                            :class:`GTVFIntegrator`, :class:`CRKSPHIntegrator`
 NNPS (LinkedListNNPS)       :class:`B200NNPS`
 DeviceHelper (``pa.gpu``)   :class:`B200DeviceHelper` / :class:`B200Backend`
 Equation / Group            :mod:`pysph_b200.equations`
 WCSPHScheme.get_equations   :class:`pysph_b200.scheme.WCSPHScheme`
 IISPHScheme.get_equations   :class:`pysph_b200.iisph.IISPHScheme`
 GTVFScheme.get_equations    :class:`pysph_b200.gtvf.GTVFScheme` (a MultiStageEquations)
+CRKSPHScheme.get_equations  :class:`pysph_b200.crksph.CRKSPHScheme` (a MultiStageEquations)
 Solver step loop            :class:`B200Solver`
 solver tools                :class:`DensityCorrection`, :class:`ShiftPositions`
 tools.interpolator          :class:`Interpolator`
@@ -55,6 +56,8 @@ from .iisph import (IISPHScheme, IISPHStep, get_particle_array_iisph, make_iisph
 from .equations import MultiStageEquations
 from .gtvf import (GTVFScheme, GTVFStep, GTVFIntegrator, get_particle_array_gtvf,
                    make_gtvf_solver)
+from .crksph import (CRKSPHScheme, CRKSPHStep, CRKSPHIntegrator, get_particle_array_crksph,
+                     make_crksph_solver)
 
 __version__ = '0.1.0'
 

@@ -49,6 +49,12 @@ IISPH_PROP_IDS.update((n, 140 + i) for i, n in enumerate(
 # 'rhodiv' and are no wall) keep p in the fp64 B200SPH_PF and rho0 in B200SPH_RHO0; GTVF walls use
 # EDAC_WALL_PROP_IDS
 GTVF_PROP_IDS = dict(PROP_IDS, p=30, rhodiv=131, p0=132)
+# conservative reproducing-kernel SPH extension (B200SPH_CRK_E ...); CRKSPH fluids (they own 'ae'
+# and 'gradbi') keep p in the fp64 B200SPH_PF.  The strided bi, gradai, gradbi and gradv take one
+# id per component (CRKSPH_STRIDED_IDS), indexed with stride dim on the host as the reference does
+CRKSPH_PROP_IDS = dict(PROP_IDS, p=30, e=160, ae=161, cs=162, V=163, ai=164, au=165, av=166,
+                       aw=167)
+CRKSPH_STRIDED_IDS = {'bi': 168, 'gradai': 171, 'gradbi': 174, 'gradv': 183}
 INT_PROP_IDS = {'gid': 64, 'tag': 65, 'pid': 66}
 USER_PROP0, MAX_USER_PROPS = 110, 16     # B200SPH_USER0, B200SPH_MAX_USER
 F64_DEVICE_PROPS = ('x', 'y', 'z', 'u', 'v', 'w', 'rho', 'h', 'm',
@@ -123,6 +129,15 @@ class GtvfProgram(C.Structure):
                 ('rho0', C.c_double), ('pref', C.c_double),
                 ('c0', C.c_double), ('alpha', C.c_double), ('nu', C.c_double),
                 ('gx', C.c_double), ('gy', C.c_double), ('gz', C.c_double)]
+
+
+class CrksphProgram(C.Structure):
+    _fields_ = [('fluid_mask', C.c_uint32), ('reserved', C.c_uint32), ('gamma', C.c_double),
+                ('gx', C.c_double), ('gy', C.c_double), ('gz', C.c_double),
+                ('cl', C.c_double), ('cq', C.c_double), ('eta_crit', C.c_double),
+                ('eta_fold', C.c_double), ('cl_e', C.c_double), ('cq_e', C.c_double),
+                ('eta_crit_e', C.c_double), ('eta_fold_e', C.c_double),
+                ('nu', C.c_double), ('eta', C.c_double)]
 
 
 class GridInfo(C.Structure):
@@ -213,6 +228,9 @@ SIGNATURES = {
     'b200sph_gtvf_pass': (C.c_int, [_ctx_p, C.POINTER(GtvfProgram), C.c_int]),
     'b200sph_stage_gtvf': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_double]),
     'b200sph_stage_gtvf_dev': (C.c_int, [_ctx_p, C.c_int, C.c_int]),
+    'b200sph_crksph_pass': (C.c_int, [_ctx_p, C.POINTER(CrksphProgram), C.c_int]),
+    'b200sph_stage_crksph': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_double]),
+    'b200sph_stage_crksph_dev': (C.c_int, [_ctx_p, C.c_int, C.c_int]),
     'b200sph_stage': (C.c_int, [_ctx_p, C.c_int, C.c_int, C.c_double]),
     'b200sph_dt_factors': (C.c_int, [_ctx_p, _dp]),
     'b200sph_time_control': (C.c_int, [_ctx_p, C.c_void_p, C.POINTER(C.c_void_p)]),

@@ -58,6 +58,9 @@ class B200AccelerationEval(object):
         self._rhotmp = self.backend.add_user_property('rhotmp') \
             if _has_op(self.ops, 'dfilter') else None
         self._kid = kernel_id(kernel)
+        # a CRKSPH evaluation fixes the host layout of the strided properties (stride dim)
+        if _has_op(self.ops, 'crksph'):
+            self.backend.strided_dim = int(kernel.dim)
         self._range = None
         self.nnps = None
         self.count_pairs = False
@@ -167,6 +170,8 @@ class B200AccelerationEval(object):
                 self._pairs += cnt.value if self.count_pairs else 0
             elif kind == 'gtvf':
                 ctx.call('b200sph_gtvf_pass', C.byref(op[1]), op[2])
+            elif kind == 'crksph':
+                ctx.call('b200sph_crksph_pass', C.byref(op[1]), op[2])
             elif kind == 'update_nnps':
                 # mako:139-145: nnps.update_domain(); nnps.update()
                 ctx.call('b200sph_update_domain')

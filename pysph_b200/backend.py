@@ -13,7 +13,12 @@ import numpy as np
 
 from . import _lib
 from ._lib import (PROP_IDS, INT_PROP_IDS, EDAC_PROP_IDS, EDAC_WALL_PROP_IDS,
-                   ELASTIC_PROP_IDS, IISPH_PROP_IDS, GTVF_PROP_IDS)
+                   ELASTIC_PROP_IDS, IISPH_PROP_IDS, GTVF_PROP_IDS, CRKSPH_PROP_IDS,
+                   CRKSPH_STRIDED_IDS)
+
+
+def _is_crksph(pa):
+    return 'ae' in pa.properties and 'gradbi' in pa.properties
 
 
 def _host_array(pa, name):
@@ -81,8 +86,12 @@ class B200Backend(object):
                               (EDAC_PROP_IDS if 'ap' in pa.properties else
                                (ELASTIC_PROP_IDS if 's00' in pa.properties else
                                 (IISPH_PROP_IDS if 'uadv' in pa.properties else
-                                 (GTVF_PROP_IDS if 'rhodiv' in pa.properties else PROP_IDS)))))
+                                 (GTVF_PROP_IDS if 'rhodiv' in pa.properties else
+                                  (CRKSPH_PROP_IDS if _is_crksph(pa) else PROP_IDS))))))
                          for pa in particle_arrays]
+        # the dimension a CRKSPH evaluation indexes the strided properties with (set when one is
+        # translated); until then they stay on the host
+        self.strided_dim = None
         self.user_props = []      # names of the fp64 properties created for generic equations
         for pa in particle_arrays:
             n = pa.get_number_of_particles()
@@ -155,7 +164,31 @@ class B200Backend(object):
                 self.ctx.call('b200sph_push_u32', i, INT_PROP_IDS[name],
                               a.ctypes.data, 0, n)
             # properties the hot path never touches (div, ...) stay host-only
+        for name, view, pid in self._strided(pa, props, n):
+            a = np.ascontiguousarray(view, dtype=np.float64)
+            self.ctx.call('b200sph_push_f64', i, pid, a.ctypes.data, 0, n)
         self._dt_cache = None
+
+    def _strided(self, pa, props, n):
+        """(name, host view, device id) of every component of the CRKSPH strided properties
+        named (all with props None): component k of dim-strided bi / gradai is bi[d i + k], of
+        gradbi / gradv (g, a) is gradbi[d d i + d g + a], at device id base + k or base + 3 g + a
+        (crksph.py:154-167)"""
+        d = self.strided_dim
+        if d is None or not _is_crksph(pa):
+            return []
+        out = []
+        for name, base in CRKSPH_STRIDED_IDS.items():
+            if name not in pa.properties or (props is not None and name not in props):
+                continue
+            a = _host_array(pa, name)
+            if name in ('bi', 'gradai'):
+                comps = [(base + k, k, d) for k in range(d)]
+            else:
+                comps = [(base + 3 * g + k, d * g + k, d * d) for g in range(d) for k in range(d)]
+            for pid, off, stride in comps:
+                out.append((name, a[off:off + stride * n:stride], pid))
+        return out
 
     def pull(self, i, props=None):
         pa = self.particle_arrays[i]
@@ -183,6 +216,10 @@ class B200Backend(object):
                 self.ctx.call('b200sph_pull_u32', i, INT_PROP_IDS[name],
                               tmp.ctypes.data, 0, n)
                 a[:] = tmp.view(a.dtype) if a.dtype.itemsize == 4 else tmp
+        for name, view, pid in self._strided(pa, props, n):
+            tmp = np.empty(n, dtype=np.float64)
+            self.ctx.call('b200sph_pull_f64', i, pid, tmp.ctypes.data, 0, n)
+            view[:] = tmp
 
     def _real_view(self, pa, name, n_real, who):
         """A contiguous fp64 host buffer of at least n_real elements, or an error: the

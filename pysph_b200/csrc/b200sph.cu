@@ -22,7 +22,7 @@
 // One translation unit: this file holds the context, the pool and every C-ABI entry
 // point; the kernels are included below by family (pool_kernels, scan, nnps_kernels,
 // sph_kernels, pair_kernel, pair_list, tvf_kernels, solid_kernels, halo_kernels, density_filter,
-// interp_kernels, shift_kernels, iisph_kernels, gtvf_kernels .cuh).
+// interp_kernels, shift_kernels, iisph_kernels, gtvf_kernels, crksph_kernels .cuh).
 //
 // No CPU fallback: every entry point needs a CUDA device.
 #include "b200sph.h"
@@ -45,7 +45,7 @@
 // --------------------------------------------------------------------------
 // small helpers
 // --------------------------------------------------------------------------
-#define N_PROP_SLOTS (B200SPH_IISPH_V + 1)   // property ids 0 .. the last IISPH property
+#define N_PROP_SLOTS (B200SPH_CRK_LAST + 1)   // property ids 0 .. the last CRKSPH property
 #define PT_INVALID 0xFFu
 #define PT_GHOST 0x08u
 
@@ -437,6 +437,8 @@ struct b200sph_ctx {
     // [n_sorted].  gtvf_spec: an evaluation 1 ran on a deferred drift check not yet confirmed;
     // gtvf_restore: that check failed, so the repeat keeps rho0 (the density of stage 2)
     Buf<ShiftRec> gtvf_P;
+    // conservative reproducing-kernel SPH (b200sph_crksph_pass): the position records [n_sorted]
+    Buf<ShiftRec> crk_P;
     bool gtvf_spec = false, gtvf_restore = false;
     // Group(start_idx, stop_idx): one-shot destination ranges of the next pair pass
     int64_t dst_lo[B200SPH_MAX_ARRAYS] = {0}, dst_hi[B200SPH_MAX_ARRAYS] = {0};
@@ -724,6 +726,7 @@ __device__ __forceinline__ void rec32_make(const float4 A, const double u, const
 #include "shift_kernels.cuh"
 #include "iisph_kernels.cuh"
 #include "gtvf_kernels.cuh"
+#include "crksph_kernels.cuh"
 
 // --------------------------------------------------------------------------
 // host side
@@ -734,7 +737,7 @@ __device__ __forceinline__ void rec32_make(const float4 A, const double u, const
 // time any IISPH property is named, or one by one when a
 // user property is named.  The only host code that knows the ranges of the id enum.
 enum PropType { PROP_NONE, PROP_F64, PROP_F32, PROP_U32 };
-enum PropGroup { GROUP_POOL, GROUP_ELASTIC, GROUP_IISPH, GROUP_GTVF, GROUP_USER };
+enum PropGroup { GROUP_POOL, GROUP_ELASTIC, GROUP_IISPH, GROUP_GTVF, GROUP_CRKSPH, GROUP_USER };
 struct PropKind {
     PropType type;
     PropGroup group;
@@ -751,6 +754,7 @@ static PropKind prop_kind(int p)
     if (p >= B200SPH_V00 && p <= B200SPH_AS22) return {PROP_F32, GROUP_ELASTIC};
     if (p >= B200SPH_UADV && p <= B200SPH_IISPH_V) return {PROP_F64, GROUP_IISPH};
     if (p >= B200SPH_RHODIV && p <= B200SPH_GTVF_P0) return {PROP_F64, GROUP_GTVF};
+    if (p >= B200SPH_CRK_E && p <= B200SPH_CRK_LAST) return {PROP_F64, GROUP_CRKSPH};
     if (p >= B200SPH_USER0 && p < B200SPH_USER0 + B200SPH_MAX_USER) return {PROP_F64, GROUP_USER};
     return {PROP_NONE, GROUP_POOL};
 }
@@ -3596,6 +3600,136 @@ static int stage_gtvf_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool
 }
 int b200sph_stage_gtvf(b200sph_ctx *ctx, int arr, int which, double dt) { return stage_gtvf_impl(ctx, arr, which, dt, false); }
 int b200sph_stage_gtvf_dev(b200sph_ctx *ctx, int arr, int which) { return stage_gtvf_impl(ctx, arr, which, 0.0, true); }
+
+// ---- conservative reproducing-kernel SPH (crksph_kernels.cuh) ----------------------------------
+// A list consumer like the GTVF pass.  Evaluation 0 runs on a deferred drift check after stage 3
+// moved the particles; everything it reads besides positions, velocities and e is written by an
+// earlier pass of the same evaluation (the first StateEquation's p and cs are overwritten before
+// anything reads them), so a repeat after a failed check needs nothing restored.  Evaluation 1
+// follows stage 2, which moves no particle, and writes ae only.
+int b200sph_crksph_pass(b200sph_ctx *ctx, const b200sph_crksph_program *prog, int evaluation)
+{
+    CU(cudaSetDevice(ctx->device));
+    int rc = ensure_pool(ctx);
+    if (rc) return rc;
+    const unsigned fm = prog->fluid_mask;
+    if (evaluation != 0 && evaluation != 1) return set_err(ctx, "crksph_pass: evaluation must be 0 or 1 (got %d)", evaluation);
+    if (fm == 0 || fm >= (1u << ctx->narr) || (fm & (fm - 1)))
+        return set_err(ctx, "crksph_pass: bad fluid mask 0x%x (one fluid array)", fm);
+    if (ctx->dim < 2) return set_err(ctx, "crksph_pass: CRKSPH runs in 2-D and 3-D");
+    if (ctx->peer_box || ctx->comm_pending) return set_err(ctx, "crksph_pass runs on one GPU (no slab decomposition)");
+    if (mirror_any(ctx)) return set_err(ctx, "crksph_pass: mirror domains are not supported");
+    for (int a = 0; a < ctx->narr; a++)
+        if (ctx->arr[a].n != ctx->arr[a].n_real)
+            return set_err(ctx, "crksph_pass: array '%s' has ghost particles", ctx->arr[a].name.c_str());
+    if (!ctx->grid_valid) return set_err(ctx, "crksph_pass: the NNPS is stale (particles were pushed, resized or moved); call nnps_update first");
+    if ((rc = ensure_prop(ctx, B200SPH_CRK_E))) return rc;
+    if ((rc = eos_flush(ctx)) || (rc = ab_positions(ctx))) return rc;
+    if (ctx->n_sorted == 0) return 0;
+    unsigned long long want[B200SPH_MAX_ARRAYS] = {0};
+    for (int a = 0; a < ctx->narr; a++)
+        if ((fm >> a) & 1u) want[a] = 0xFFull << (8 * a);
+    if ((rc = prepare_lists(ctx, want, "crksph_pass: the neighbour lists cannot index the particles"))) return rc;
+    const size_t n = (size_t)ctx->n_sorted;
+    if ((rc = grow(ctx, ctx->crk_P, n, n))) return rc;
+    CrkArgs ca;
+    memset(&ca, 0, sizeof(ca));
+    ca.P = ctx->crk_P;
+    ca.perm = ctx->perm; ca.cnt = ctx->cnt; ca.lst = ctx->lst; ca.skey = ctx->skey; ca.stype = ctx->stype;
+    ca.h = f64_ptr(ctx, B200SPH_H); ca.m = f64_ptr(ctx, B200SPH_M);
+    ca.u = f64_ptr(ctx, B200SPH_U); ca.v = f64_ptr(ctx, B200SPH_V); ca.w = f64_ptr(ctx, B200SPH_W);
+    ca.u0 = f64_ptr(ctx, B200SPH_U0); ca.v0 = f64_ptr(ctx, B200SPH_V0); ca.w0 = f64_ptr(ctx, B200SPH_W0);
+    ca.rho = f64_ptr(ctx, B200SPH_RHO); ca.p = f64_ptr(ctx, B200SPH_PF);
+    ca.e = f64_ptr(ctx, B200SPH_CRK_E); ca.ae = f64_ptr(ctx, B200SPH_CRK_AE); ca.cs = f64_ptr(ctx, B200SPH_CRK_CS);
+    ca.V = f64_ptr(ctx, B200SPH_CRK_V); ca.ai = f64_ptr(ctx, B200SPH_CRK_AI);
+    ca.au = f64_ptr(ctx, B200SPH_CRK_AU); ca.av = f64_ptr(ctx, B200SPH_CRK_AV); ca.aw = f64_ptr(ctx, B200SPH_CRK_AW);
+    for (int k = 0; k < 3; k++) {
+        ca.bi[k] = f64_ptr(ctx, B200SPH_CRK_BI0 + k);
+        ca.gai[k] = f64_ptr(ctx, B200SPH_CRK_GRADAI0 + k);
+    }
+    for (int k = 0; k < 9; k++) {
+        ca.gbi[k] = f64_ptr(ctx, B200SPH_CRK_GRADBI00 + k);
+        ca.gv[k] = f64_ptr(ctx, B200SPH_CRK_GRADV00 + k);
+    }
+    ca.n = ctx->n_sorted; ca.capg = ctx->capg;
+    ca.ncx = ctx->G.nc[0]; ca.ncy = ctx->G.nc[1]; ca.zorder = ctx->G.zorder;
+    for (int d = 0; d < 3; d++) {
+        ca.per[d] = ctx->G.periodic[d];
+        ca.L[d] = ctx->dom_hi[d] - ctx->dom_lo[d];
+    }
+    ca.kr = ctx->radius_scale;
+    ca.kfac = kernel_fac(ctx->kernel, ctx->dim);
+    ca.fluid_mask = fm;
+    ca.gamma = prog->gamma; ca.gx = prog->gx; ca.gy = prog->gy; ca.gz = prog->gz;
+    ca.cl = prog->cl; ca.cq = prog->cq; ca.eta_crit = prog->eta_crit; ca.eta_fold = prog->eta_fold;
+    ca.cl_e = prog->cl_e; ca.cq_e = prog->cq_e; ca.eta_crit_e = prog->eta_crit_e; ca.eta_fold_e = prog->eta_fold_e;
+    ca.nu = prog->nu; ca.eta = prog->eta;
+    PhaseTimer pt(ctx, 2);
+    k_crksph_pack<<<(unsigned)cdiv(ctx->n_sorted, 256), 256, 0, ctx->stream>>>(
+        ca, f64_ptr(ctx, B200SPH_X), f64_ptr(ctx, B200SPH_Y), f64_ptr(ctx, B200SPH_Z));
+    LAUNCH_CHECK();
+    const unsigned nb = (unsigned)cdiv(ctx->n_sorted, CRK_NT);
+    const auto pass = [&](const int which) {
+        return with_kernel_dim(ctx, "crksph_pass", [&](auto kc, auto dc) {
+            constexpr int K = decltype(kc)::value, D = decltype(dc)::value;
+            if constexpr (D >= 2) {
+                switch (which) {
+                case CRK_VOL: k_crksph<K, D, CRK_VOL><<<nb, CRK_NT, 0, ctx->stream>>>(ca); break;
+                case CRK_PRE: k_crksph<K, D, CRK_PRE><<<nb, CRK_NT, 0, ctx->stream>>>(ca); break;
+                case CRK_RHO: k_crksph<K, D, CRK_RHO><<<nb, CRK_NT, 0, ctx->stream>>>(ca); break;
+                case CRK_GRADV: k_crksph<K, D, CRK_GRADV><<<nb, CRK_NT, 0, ctx->stream>>>(ca); break;
+                case CRK_MOM: k_crksph<K, D, CRK_MOM><<<nb, CRK_NT, 0, ctx->stream>>>(ca); break;
+                default: k_crksph<K, D, CRK_ENERGY><<<nb, CRK_NT, 0, ctx->stream>>>(ca); break;
+                }
+                LAUNCH_CHECK();
+            }
+            return 0;
+        });
+    };
+    if (evaluation == 0) {
+        for (const int which : {CRK_VOL, CRK_PRE, CRK_RHO, CRK_GRADV, CRK_MOM})
+            if ((rc = pass(which))) return rc;
+    } else if ((rc = pass(CRK_ENERGY))) {
+        return rc;
+    }
+    ctx->stats.pair_launches++;
+    pt.stop();
+    state_changed(ctx);
+    ctx->spec_records = false;
+    return 0;
+}
+
+static int stage_crksph_impl(b200sph_ctx *ctx, int arr, int which, double dt, bool devdt)
+{
+    int rc = stage_begin(ctx, "stage_crksph", arr, which, devdt, 3);
+    if (rc) return rc;
+    if (which < 1) return set_err(ctx, "stage_crksph: CRKSPHStep has stages 1, 2 and 3 (got %d)", which);
+    if ((rc = ensure_prop(ctx, B200SPH_CRK_E))) return rc;
+    PhaseTimer pt(ctx, 2);
+    StageCrkArgs sa;
+    sa.x = f64_ptr(ctx, B200SPH_X); sa.y = f64_ptr(ctx, B200SPH_Y); sa.z = f64_ptr(ctx, B200SPH_Z);
+    sa.u = f64_ptr(ctx, B200SPH_U); sa.v = f64_ptr(ctx, B200SPH_V); sa.w = f64_ptr(ctx, B200SPH_W);
+    sa.u0 = f64_ptr(ctx, B200SPH_U0); sa.v0 = f64_ptr(ctx, B200SPH_V0); sa.w0 = f64_ptr(ctx, B200SPH_W0);
+    sa.e = f64_ptr(ctx, B200SPH_CRK_E); sa.ae = f64_ptr(ctx, B200SPH_CRK_AE);
+    sa.au = f64_ptr(ctx, B200SPH_CRK_AU); sa.av = f64_ptr(ctx, B200SPH_CRK_AV); sa.aw = f64_ptr(ctx, B200SPH_CRK_AW);
+    sa.ptype = ctx->ptype;
+    sa.pool_end = ctx->pool_end;
+    sa.mask = arr < 0 ? ~0u : 1u << arr;
+    sa.which = which;
+    sa.dt = dt;
+    sa.tc = devdt ? ctx->tc : nullptr;
+    if (ctx->pool_end > 0) {
+        k_stage_crksph<<<(unsigned)cdiv(ctx->pool_end, 256), 256, 0, ctx->stream>>>(sa);
+        LAUNCH_CHECK();
+    }
+    // only stage 3 moves particles: after stages 1 and 2 the lists stay valid for the evaluation
+    // that follows
+    if (which == 3) particles_moved(ctx);
+    else state_changed(ctx);
+    return 0;
+}
+int b200sph_stage_crksph(b200sph_ctx *ctx, int arr, int which, double dt) { return stage_crksph_impl(ctx, arr, which, dt, false); }
+int b200sph_stage_crksph_dev(b200sph_ctx *ctx, int arr, int which) { return stage_crksph_impl(ctx, arr, which, 0.0, true); }
 
 // the fused stage kernel applies when one launch steps every array (arr == -1) and the
 // neighbour lists of the current build can be reused: then the records of the next

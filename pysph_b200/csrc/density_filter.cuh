@@ -52,10 +52,11 @@ __global__ void k_dfilter_pack(const DensityFilterArgs a)
     a.F[2 * s + 1] = make_float4((float)m, v, __int_as_float(t), 0.0f);
 }
 
-// gj_solve (linalg.py:94-166) on [A | e0] in its operation order.  Its pivot search swaps an
-// element with itself, so this is elimination without pivoting.  false: one of its two early
-// returns, which leave the caller's result at e0.
-template <int N> __device__ __forceinline__ bool gj_solve(double (&m)[N][N + 1])
+// gj_solve (linalg.py:94-166) on [A | B], NB right-hand-side columns, in its operation order.  Its
+// pivot search swaps an element with itself, so this is elimination without pivoting.  false: one
+// of its two early returns, which leave the caller's result as it was (the back substitution tests
+// the last column only, as the reference does).
+template <int N, int NB = 1> __device__ __forceinline__ bool gj_solve(double (&m)[N][N + NB])
 {
 #pragma unroll
     for (int c = 0; c < N; c++)
@@ -65,19 +66,19 @@ template <int N> __device__ __forceinline__ bool gj_solve(double (&m)[N][N + 1])
             if (fabs(d) < 1e-12) return false;
             const double cc = -m[r][c] / d;
 #pragma unroll
-            for (int j = 0; j <= N; j++) m[r][j] = m[r][j] + cc * m[c][j];
+            for (int j = 0; j < N + NB; j++) m[r][j] = m[r][j] + cc * m[c][j];
         }
 #pragma unroll
     for (int rb = N - 1; rb >= 0; rb--) {
         if (m[rb][rb] == 0.0) {
-            if (fabs(m[rb][N]) > 1e-12) return false;
+            if (fabs(m[rb][N + NB - 1]) > 1e-12) return false;
         } else {
 #pragma unroll
-            for (int bc = N; bc >= rb; bc--) m[rb][bc] = m[rb][bc] / m[rb][rb];
+            for (int bc = N + NB - 1; bc >= rb; bc--) m[rb][bc] = m[rb][bc] / m[rb][rb];
 #pragma unroll
             for (int ku = rb - 1; ku >= 0; ku--)
 #pragma unroll
-                for (int kl = N; kl >= rb; kl--) {
+                for (int kl = N + NB - 1; kl >= rb; kl--) {
                     const double kk = -m[ku][rb] / m[rb][rb];
                     m[ku][kl] = m[ku][kl] + kk * m[rb][kl];
                 }

@@ -39,6 +39,7 @@ _SUPPORTED_STEPPERS = {
     'WCSPHTVDRK3Step': ('b200sph_stage_rk3', 'b200sph_stage_rk3_dev'),
     'IISPHStep': ('b200sph_stage_iisph', 'b200sph_stage_iisph_dev'),   # iisph.py:22-34
     'GTVFStep': ('b200sph_stage_gtvf', 'b200sph_stage_gtvf_dev'),      # wc/gtvf.py:70-98
+    'CRKSPHStep': ('b200sph_stage_crksph', 'b200sph_stage_crksph_dev'),   # wc/crksph.py:884-900
 }
 
 

@@ -14,6 +14,7 @@ recognises each equation by *class name* and maps every Group onto
     ('correct_vel', array_mask)                            CorrectVelocities after a shift
     ('iisph', IisphProgram, fluid_indices)                 IISPHScheme's Groups, as a whole
     ('gtvf', GtvfProgram, evaluation)                      one evaluation of GTVFScheme, as a whole
+    ('crksph', CrksphProgram, evaluation)                  one evaluation of CRKSPHScheme, as a whole
 
 Anything the CUDA library has no kernel for raises NotImplementedError here,
 i.e. at setup time, never silently at run time.
@@ -453,7 +454,8 @@ def build_program(groups, array_names, dim, particle_arrays=None, kernel=None, g
     groups = group_equations(groups)
     i = 0
     while i < len(groups):
-        found = _match_iisph(groups, i, index) or _match_gtvf(groups, i, index, arrays)
+        found = _match_iisph(groups, i, index) or _match_gtvf(groups, i, index, arrays) or \
+            _match_crksph(groups, i, index)
         if found:
             ops.append(found[0])
             i += found[1]
@@ -615,6 +617,85 @@ def _match_gtvf(groups, i, index, arrays):
         for k in ('rho0', 'pref', 'c0', 'alpha', 'nu', 'gx', 'gy', 'gz'):
             setattr(prog, k, float(kw.get(k, 0.0)))
         return ('gtvf', prog, evaluation), n
+    return None
+
+
+# ---- CRKSPHScheme (pysph/sph/wc/crksph.py:978-1127) -------------------------------------------
+_CRKSPH_PARAMS = ('dim', 'gamma', 'gx', 'gy', 'gz', 'cl', 'cq', 'eta_crit', 'eta_fold', 'tol', 'nu',
+                  'eta')
+
+
+def _crksph_signature(g):
+    """What must agree between a Group and the one CRKSPHScheme.get_equations emits: the flags and,
+    per equation, its class, whether its module is crksph (MomentumEquation and StateEquation
+    share names with other families), destination, sources and parameters."""
+    flags = (bool(getattr(g, 'real', True)), bool(getattr(g, 'iterate', False)),
+             bool(getattr(g, 'update_nnps', False)), getattr(g, 'pre', None) is None,
+             getattr(g, 'post', None) is None, getattr(g, 'condition', None) is None,
+             getattr(g, 'start_idx', 0) in (0, None), getattr(g, 'stop_idx', None) is None,
+             bool(getattr(g, 'has_subgroups', False)))
+    if flags[-1]:
+        return flags
+    eqs = []
+    for eq in g.equations:
+        eqs.append((_eq_name(eq), 'crksph' in eq.__class__.__module__, eq.dest,
+                    tuple(eq.sources or ())) +
+                   tuple((k, float(getattr(eq, k))) for k in _CRKSPH_PARAMS if hasattr(eq, k)))
+    return flags + (tuple(eqs),)
+
+
+def _match_crksph(groups, i, index):
+    """(('crksph', CrksphProgram, evaluation), number of Groups) when groups[i:] is one of the two
+    evaluations CRKSPHScheme.get_equations emits, with or without has_ghosts -- the same Groups,
+    in the same order, for the fluids and parameters they name -- else None.  Several fluid arrays
+    are refused here."""
+    from .crksph import CRKSPHScheme
+    for evaluation, ghosts, n in ((0, True, 12), (0, False, 8), (1, True, 2), (1, False, 1)):
+        gs = groups[i:i + n]
+        if len(gs) != n:
+            continue
+        try:
+            if evaluation == 0:
+                eos = [eq for eq in gs[0].equations if _eq_name(eq) == 'StateEquation']
+                fluids = [eq.dest for eq in eos]
+                mom = [eq for eq in gs[-1].equations if _eq_name(eq) == 'MomentumEquation'][0]
+                sym = gs[-1].equations[0]
+                visc = [eq for eq in gs[-1].equations if _eq_name(eq) == 'LaminarViscosity']
+                kw = dict(dim=int(mom.dim), gamma=float(eos[0].gamma), gx=float(mom.gx),
+                          gy=float(mom.gy), gz=float(mom.gz), cl=float(mom.cl), cq=float(mom.cq),
+                          eta_crit=float(mom.eta_crit), eta_fold=float(mom.eta_fold),
+                          tol=float(sym.tol), nu=float(visc[0].nu) if visc else 0.0)
+                eta = float(visc[0].eta) if visc else 0.01
+            else:
+                en = [eq for eq in gs[-1].equations if _eq_name(eq) == 'EnergyEquation']
+                fluids = [eq.dest for eq in en]
+                sym = gs[-1].equations[0]
+                kw = dict(dim=int(en[0].dim), gamma=float(en[0].gamma), tol=float(sym.tol), nu=0.0)
+            want = CRKSPHScheme(fluids, rho0=1.0, c0=1.0, h0=1.0, p0=0.0, has_ghosts=ghosts,
+                                **kw).get_equations().groups[evaluation]
+            if len(want) != n or any(_crksph_signature(a) != _crksph_signature(b)
+                                     for a, b in zip(gs, want)):
+                continue
+        except (AttributeError, IndexError, TypeError, ValueError):
+            continue
+        if any(a not in index for a in fluids):
+            raise ValueError('CRKSPHScheme: unknown particle array among %r' % fluids)
+        if len(fluids) != 1:
+            raise NotImplementedError(
+                'B200 backend: CRKSPHScheme with %d fluid arrays (the reference\'s '
+                'CRKSPHPreStep.loop_all keeps the moments of the last source only); one fluid '
+                'array is supported' % len(fluids))
+        prog = _lib.CrksphProgram()
+        prog.fluid_mask = 1 << index[fluids[0]]
+        prog.gamma = kw['gamma']
+        if evaluation == 0:
+            for k in ('gx', 'gy', 'gz', 'cl', 'cq', 'eta_crit', 'eta_fold', 'nu'):
+                setattr(prog, k, kw[k])
+            prog.eta = eta
+        else:
+            for k in ('cl', 'cq', 'eta_crit', 'eta_fold'):
+                setattr(prog, k + '_e', float(getattr(en[0], k)))
+        return ('crksph', prog, evaluation), n
     return None
 
 

@@ -173,6 +173,9 @@ class B200Solver(object):
                                                    getattr(dom, 'is_mirror', False)):
             raise NotImplementedError(
                 'B200 backend: periodic / mirror domains with the slab decomposition')
+        if pm is not None and any('ae' in pa.properties and 'gradbi' in pa.properties
+                                  for pa in self.particles):
+            raise NotImplementedError('B200 backend: CRKSPHScheme with the slab decomposition')
         if pm is not None and any('rhodiv' in pa.properties for pa in self.particles):
             raise NotImplementedError('B200 backend: GTVFScheme with the slab decomposition')
         if pm is not None and any('uadv' in pa.properties for pa in self.particles):
